@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- forward+backward rasterization throughput on synthetic Gaussian clouds (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One *step* = one forward + one backward rasterization of the named workload (default C3: 3M Gaussians,
@@ -20,7 +20,12 @@ Rank 0 prints ONE JSON line:
                         after the timed region) and their algorithmic bytes
   cpu_baseline          the CPU oracle (oracle/oracle.c, OpenMP) on a bounded sample of the workload, rank 0, N=1
 
---impl reference times the UNMODIFIED reference rasterizer compiled for sm_100a (oracle/_ref/libdgr_ref.so; the
+--dump-outputs DIR writes what the timed path returned in its last timed step (image, radii, every gradient) as
+float32 DIR/<name>.npy: arrays with one row per Gaussian on a fixed seeded sample of rows, arrays above 8 M elements
+on a fixed seeded sample of elements (<= 64 MB in all).  Inputs are seeded, so two builds run with the same arguments
+can be compared output for output.
+
+--impl reference times the UNMODIFIED reference rasterizer compiled for sm_90a (oracle/_ref/libdgr_ref.so; the
 reference has no CPU implementation of this path, its own implementation IS CUDA) on the same tensors; if that
 library did not travel with the snapshot it falls back to the CPU oracle port.  Rank 0 only.
 """
@@ -45,7 +50,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import synthetic  # noqa: E402
 
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0     # H100 SXM data sheet (HBM3), for a card allowed 700 W
 E2E_NOTE = ("value / ms_per_step = the FASTEST of the forms below (both arms).  ms_per_step_pipelined: public API (GaussianRasterizer + autograd) on pinned HOST buffers, every step copies all of its "
             "inputs host->device and its image + all gradients device->host inside the timed region; steps are software-pipelined "
             "(<= 3 in flight: step i's read-back overlaps step i+1's uploads on the other PCIe direction; the closing event waits "
@@ -64,19 +69,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(kernel, config):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the committed `ncu --set full`
-    capture of this workload (profiles/ncu_traffic.json); None when no capture of that kernel/config is committed."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        if t.get("config", "C3") != config:
-            return None
-        return t["dram_bytes_per_launch"].get(kernel)
-    except Exception:
-        return None
+    return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -123,6 +116,30 @@ class ClockSampler:
         busy = [s for s in sm if s > 0]
         return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+DUMP_ROWS = 65536              # per-Gaussian rows kept by --dump-outputs
+DUMP_MAX_ELEMS = 8 * 1024 * 1024
+
+
+def dump_outputs(out_dir, P, arrays):
+    """Writes `arrays` ({name: tensor or None}) as float32 .npy files under `out_dir`, sampled as the module doc says."""
+    os.makedirs(out_dir, exist_ok=True)
+    rows = np.sort(np.random.default_rng(2024).choice(P, size=min(P, DUMP_ROWS), replace=False)) if P else None
+    for name, t in arrays.items():
+        if t is None or t.numel() == 0:
+            continue
+        a = t.detach().float().cpu().numpy()
+        if a.ndim >= 1 and a.shape[0] == P and P > DUMP_ROWS:
+            a = a[rows]
+        elif a.size > DUMP_MAX_ELEMS:
+            a = a.reshape(-1)[np.sort(np.random.default_rng(2025).choice(a.size, size=DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
+def step_outputs(color, radii, grads):
+    from golden_util import GRAD_NAMES
+    return dict({"out_color": color, "radii": radii}, **dict(zip(GRAD_NAMES, grads)))
 
 
 def call_args(d):
@@ -468,6 +485,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-train-step", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32, sampled, <= 64 MB)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
 
@@ -499,7 +518,7 @@ def main():
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic (seeded, SURVEY.md 8d generator)",
             "config": {"workload": workload, "P": P, "W": W, "H": H, "tiles": T,
-                       "l2": "inputs_larger_than_l2 (per-step working set >= 0.5 GB vs 126 MB L2)",
+                       "l2": "inputs_larger_than_l2 (per-step working set >= 0.5 GB vs 50 MB L2)",
                        "parallelism": "single GPU" if world == 1 else f"tile-row bands x{world}, " + {
                            "0": "NCCL all-gather (image) + all-reduce (partials)",
                            "1": "image all-gather fused into the forward composite (peer stores) and partial-gradient reduction fused "
@@ -518,13 +537,18 @@ def main():
         line["impl"] = "reference"
         if ref_cuda.available():
             mod = ref_cuda
+            last = {}
             def step():
                 R, color, radii, geom, binning, img = mod.rasterize_gaussians(*call_args(d))
-                mod.rasterize_gaussians_backward(*backward_args(d, radii, geom, R, binning, img))
+                grads = mod.rasterize_gaussians_backward(*backward_args(d, radii, geom, R, binning, img))
+                last.update(out=(color, radii, grads))
             sampler.start()
             ms = time_steps(step, a.steps, a.warmup, dev, 1)
+            if a.dump_outputs:
+                dump_outputs(a.dump_outputs, P, step_outputs(*last["out"]))
+                last.clear()
             line.update(value=P * N / (ms * 1e-3), ms_per_step=ms,
-                        reference_kind="unmodified reference CUDA rasterizer compiled for sm_100a (oracle/_ref/libdgr_ref.so), "
+                        reference_kind="unmodified reference CUDA rasterizer compiled for sm_90a (oracle/_ref/libdgr_ref.so), "
                                        "legacy default stream, run on the GPU: the reference has no CPU implementation of this path")
             # e2e with the same host-buffer harness, through the reference's own Python surface re-created around its _C
             if not a.no_e2e:
@@ -584,7 +608,7 @@ def main():
         def step():
             R, color, radii, geom, binning, img = _C.rasterize_gaussians(*call_args(d))
             grads = _C.rasterize_gaussians_backward_lean(*backward_args(d, radii, geom, R, binning, img))
-            state.update(R=R, radii=radii, geom=geom, binning=binning, img=img)
+            state.update(R=R, radii=radii, geom=geom, binning=binning, img=img, color=color, grads=grads)
     else:
         state = {}
         def step():
@@ -618,6 +642,10 @@ def main():
     sampler.start()
     ms = time_steps(step, a.steps, a.warmup, dev, world)
     launches = (_C.launch_count() - launches0) // (a.steps + a.warmup) * a.steps
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, P, step_outputs(state["color"] if world == 1 else state["full"], state["radii"],
+                                                     state["grads"]))
+    state.pop("color", None); state.pop("grads", None); state.pop("full", None)
 
     # separate fwd / bwd times and per-stage times: K profiled steps right after the timed region
     R = state["R"]
@@ -667,7 +695,7 @@ def main():
         dom = max(stages, key=lambda k: stages[k]["ms"])
         line["stages"] = stages
         line["roofline"] = {"bound": "hbm", "kernel": dom, "achieved": stages[dom]["gbs"], "peak": peak, "unit": "GB/s",
-                            "frac": stages[dom]["gbs"] / peak, "traffic": ncu_traffic(dom, a.config), "peak_source": peak_src,
+                            "frac": stages[dom]["gbs"] / peak, "peak_source": peak_src,
                             "alg_bytes_per_launch": stages[dom]["alg_bytes"], "launch_ms": stages[dom]["ms"]}
         Bf, Bb = path_bytes(P, V, R, N, sh_M)
         # second reading: the formula charges R * (36 + 40) B of per-instance delivery, but only `visited` of the R list
@@ -705,7 +733,7 @@ def main():
             dom = max(stages, key=lambda k: stages[k]["ms"])
             line["stages"] = stages
             line["roofline"] = {"bound": "hbm", "kernel": dom, "rank": 0, "achieved": stages[dom]["gbs"], "peak": peak,
-                                "unit": "GB/s", "frac": stages[dom]["gbs"] / peak, "traffic": None, "peak_source": peak_src,
+                                "unit": "GB/s", "frac": stages[dom]["gbs"] / peak, "peak_source": peak_src,
                                 "alg_bytes_per_launch": stages[dom]["alg_bytes"], "launch_ms": stages[dom]["ms"]}
             Bf, Bb = path_bytes(P, V, R_tot, N, sh_M)
             line["roofline_path"] = {"bound": "hbm", "B_fwd": int(Bf), "B_bwd": int(Bb),
@@ -832,7 +860,7 @@ def other_config_lines(impl_step_factory, dev, steps, peak, names=("C2", "C5")):
 
 
 def colour_op_bench(P, dev, steps):
-    """SURVEY 8f-2: the fused per-Gaussian colour op (csrc/appearance.cu, tcgen05) on P rows next to the PyTorch statements
+    """SURVEY 8f-2: the fused per-Gaussian colour op (csrc/appearance.cu, wgmma) on P rows next to the PyTorch statements
     it replaces (oracle/color_torch.py = method.py:1570-1598 in fp32), forward and forward+backward, CUDA events."""
     import fused_colors as fc
     from oracle import color_torch as ct
@@ -891,18 +919,18 @@ def colour_op_bench(P, dev, steps):
                        "fwd_frac": None if not pk else fwd_flop / (res["fused_fwd_ms"] * 1e-3) / 1e12 / pk,
                        "hbm_bytes_fwd": P * (3 + 45 + 24 + 3 + 6) * 4, "hbm_bytes_bwd": P * (3 + 45 + 24 + 3 + 6 + 3 + 45 + 24 + 3) * 4,
                        "note": "MMA flops as issued (K padded to 32 / 144, N to 16); the op is bounded by the CUDA-core epilogues "
-                               "(tcgen05.ld + ReLU + bf16 pack + SH) and by HBM, not by the tensor pipe"}
+                               "(ReLU + bf16 pack + SH) and by HBM, not by the tensor pipe"}
     return res
 
 
 def full_train_step(kw, dev, steps, impl="ours"):
     """ms per step of `GaussianModel._render_internal` + loss + backward (unmodified wildgaussians/method.py from
-    baseline/_ref, see tests/wg_harness.py) on a cloud of the workload's size with SH degree 3 + 32-d appearance
+    oracle/_ref/py, see tests/wg_harness.py) on a cloud of the workload's size with SH degree 3 + 32-d appearance
     embedding (BASELINE.json config 3), on this repo's rasterizer and on the reference's compiled CUDA core."""
     import wg_harness as wh
     m, Config = wh.import_method()
     if m is None:
-        return {"unavailable": "reference python package not present (baseline/_ref)"}
+        return {"unavailable": "reference python package not present (oracle/_ref/py)"}
     import diff_gaussian_rasterization as ours
     from oracle import ref_cuda
     kw3 = dict(kw); kw3["sh_degree"] = 3
@@ -924,7 +952,7 @@ def full_train_step(kw, dev, steps, impl="ours"):
         for name, rcls, scls in arms:
             wh.use_backend(m, rcls, scls)
             res[name] = time_steps(lambda: wh.train_step(model, cfg, cam, G1, G2), steps, 3, dev, 1)
-        # opt-in fused caller (wildgaussians_fused.enable): fused tcgen05 colour op + cached camera constants, same
+        # opt-in fused caller (wildgaussians_fused.enable): fused wgmma colour op + cached camera constants, same
         # rasterizer, method.py still unmodified
         import wildgaussians_fused as wf
         wh.use_backend(m, ours.GaussianRasterizer, ours.GaussianRasterizationSettings)

@@ -1,5 +1,5 @@
 /*
- * gsrast.h -- C ABI of libgsrast.so, the sm_100a Gaussian-splat rasterizer.
+ * gsrast.h -- C ABI of libgsrast.so, the sm_90a Gaussian-splat rasterizer.
  *
  * This header is the drop-in boundary for the hot path of jkulhanek/wild-gaussians:
  * it replaces the C++ entry points the reference's pybind11 module binds
@@ -252,7 +252,7 @@ int gsr_get_stats(const void* geom_buffer, int P, int M, void* stream, GsrStats*
  * PyTorch statements of wildgaussians/method.py that turn the model's features into the two colour sets the rasterizer
  * composites: `features.clamp_max(1)` (:1570), eval_sh + 0.5 + clamp_min(0) for the raw colours (:1571-1579, :493-548),
  * EmbeddingModel.forward (59 -> 128 -> 128 -> 6 MLP, x 0.01, affine on the features; :874-900) and the toned colours
- * (:1586-1598).  The MLP runs on tcgen05 tensor cores (bf16 operands, fp32 accumulation in TMEM).
+ * (:1586-1598).  The MLP runs on wgmma tensor cores (bf16 operands, fp32 accumulation).
  *   1. gsr_appearance_pack_weights(): fp32 nn.Linear parameters + the image embedding -> packed bf16 operand image
  *      (gsr_appearance_packed_weight_bytes() bytes, 16-byte aligned); once per step
  *   2. gsr_appearance_colors_forward():  colors_raw (optional) and colors_toned, [P,3] each

@@ -44,7 +44,7 @@ def _bf16(x):
 
 def mlp_bf16(color, embeddings, app_embedding, W1, b1, W2, b2, W3, b3):
     """The 59 -> 128 -> 128 -> 6 MLP with the OPERAND ROUNDING of csrc/appearance.cu (fp32 tensors): inputs, weights
-    and hidden activations rounded to bf16, products exact and sums in fp32 (tcgen05 kind::f16), biases kept to
+    and hidden activations rounded to bf16, products exact and sums in fp32 (wgmma bf16), biases kept to
     ~2^-17 (bias_hi + bias_lo), the image embedding folded into the first bias in fp32.  Same function as the fp32 MLP
     up to that rounding -- but its ReLU masks are those of the rounded network, which is what a gradient check of the
     kernel needs (a mask flipped by rounding changes a gradient entry by O(1): the gradient of a network with kinks

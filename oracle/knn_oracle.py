@@ -7,7 +7,7 @@ cannot contain a closer point -- so its result is a function of the point set al
 in the reference build: read off its SASS and pinned by the goldens -- any other nesting changes ~10 % of the last bits),
 summed smallest first and divided by 3.0f (:182).  This file evaluates exactly that, by brute force for small P and through
 a k-d tree candidate search (scipy) for larger P.  Pinned on the GPU box against the compiled, unmodified reference
-(oracle/_ref/libsimpleknn_ref.so, tests/test_knn.py) and here against tests/golden/knn_*.npz made by that library on a B200.
+(oracle/_ref/libsimpleknn_ref.so, tests/test_knn.py) and here against tests/golden/knn_*.npz made by that library on a GPU.
 Only tests / smoke / bench may import it."""
 from __future__ import annotations
 

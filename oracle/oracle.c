@@ -12,7 +12,7 @@
  *
  * Numerics.  The reference is compiled by nvcc with -fmad=true: products feeding sums are
  * contracted into fused multiply-adds.  The contraction pattern was read off the reference's
- * PTX/SASS (built for sm_100a, nvcc 12.9):
+ * PTX/SASS (nvcc 12.9):
  *     a*b + c*d            -> fma(a, b, rnd(c*d))        (first product fused, second rounded)
  *     (a*b + c*d) + e*f    -> fma(e, f, fma(a, b, rnd(c*d)))
  *     x + a*b, a*b + x     -> fma(a, b, x)
@@ -21,7 +21,7 @@
  * -ffp-contract=off so gcc adds none of its own).  With that, every integer artefact
  * (radii, tile rectangles, depth keys, sorted instance list, tile ranges) is bit-identical
  * to the reference's; this is pinned by tests/golden/ (vectors produced by the reference
- * itself on a B200, see tests/golden/make_golden.py).  expf() is glibc's, not CUDA's
+ * itself on a GPU, see tests/golden/make_golden.py).  expf() is glibc's, not CUDA's
  * (MUFU.EX2 based) one, so composited pixels agree to ~1e-6 and a handful of alpha-threshold
  * decisions per million may flip; tests state the tolerance.
  *

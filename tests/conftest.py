@@ -2,7 +2,7 @@
 
 * `-m "not gpu"` (runs on the CPU-only build box): oracle vs the golden vectors, host logic, the C-ABI
   library loads and exports every declared symbol, gloo world_size-2 sharding tests.
-* `-m gpu` (runs on a B200): the parity tests proper, through the C ABI / Python drop-in API.
+* `-m gpu` (runs on an H100): the parity tests proper, through the C ABI / Python drop-in API.
 """
 import os
 import sys
@@ -16,7 +16,7 @@ for p in (ROOT, os.path.join(ROOT, "wild-gaussians_b200"), os.path.join(ROOT, "t
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # Make sure the in-tree libraries are up to date BEFORE any test module imports (and dlopens) them
     # (no-op when they are newer than their sources).
     import __graft_entry__ as ge

@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference CUDA rasterizer
-(oracle/_ref/libdgr_ref.so, built by oracle/Makefile from /root/reference) on a B200.
+(oracle/_ref/libdgr_ref.so, built by oracle/Makefile from the reference checkout) on a GPU.
 
 The reference has no golden vectors of its own (SURVEY.md section 8c: "parity unpinned by the reference's
 own tests"), so these files pin the CPU oracle (tests/test_oracle_golden.py, runs without a GPU) and the

@@ -165,7 +165,7 @@ def test_adopting_the_optimizer_built_by_the_unmodified_method_py():
     import fused_adam
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     import diff_gaussian_rasterization as ours
     dev = torch.device("cuda:0")
     kw = dict(P=30_000, W=320, H=200, seed=71)

@@ -1,4 +1,4 @@
-"""GPU parity of the fused colour op (csrc/appearance.cu, tcgen05) against (a) the golden vectors produced by the
+"""GPU parity of the fused colour op (csrc/appearance.cu, wgmma) against (a) the golden vectors produced by the
 reference itself (tests/golden/colors_*.npz: outputs + autograd gradients of wildgaussians' EmbeddingModel / eval_sh in
 fp64) and (b) the torch restatement oracle/color_torch.py in fp32 on larger seeded inputs (raw + toned colours, every
 gradient incl. the mean through the view direction, ragged last tile).

@@ -73,7 +73,7 @@ def test_kernel_matches_unmodified_method_on_the_device_and_unseen_gaussians():
     import wildgaussians_fused as wf
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     dev = torch.device("cuda:0")
     P = 200_003
     cfg = Config(source_path="", model_path="", uncertainty_mode="disabled")

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on a B200 with ``-m gpu``): the CUDA path, called through the C ABI
+"""GPU parity tests (run on an H100 with ``-m gpu``): the CUDA path, called through the C ABI
 (``diff_gaussian_rasterization._C`` is a ctypes shim over ``include/gsrast.h``) and through the drop-in Python
 API, against (a) the committed golden vectors of the reference, (b) the compiled reference itself when
 ``oracle/_ref/libdgr_ref.so`` travelled with the snapshot, (c) the CPU oracle; plus size-independent

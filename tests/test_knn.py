@@ -3,7 +3,7 @@ kernels (csrc/knn.cu) behind the reference's own import path (``from simple_knn.
 
 The result is a function of the point set alone (exact 3-nearest-neighbour search, fixed fp32 expression), so the bar is
 BIT-EXACT: against the compiled unmodified reference on the same device, against golden outputs that library produced on a
-B200 (tests/golden/knn_*.npz, where present), and against the CPU oracle."""
+GPU (tests/golden/knn_*.npz, where present), and against the CPU oracle."""
 import os
 import sys
 
@@ -86,7 +86,7 @@ def test_initialize_from_points3D_of_the_unmodified_method_uses_it():
     import wg_harness as wh
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     import simple_knn._C as ours
     assert m.distCUDA2 is ours.distCUDA2
     dev = torch.device("cuda:0")

@@ -36,7 +36,7 @@ def ref_api():
 def test_render_internal_on_the_drop_in_equals_reference_backend(kw, ref_api):
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     import diff_gaussian_rasterization as ours
     from diff_gaussian_rasterization import _C
     dev = torch.device("cuda:0")
@@ -86,7 +86,7 @@ def test_fused_render_internal_matches_the_reference_method():
     that pass through the MLP in direction and size (cosine >= 0.99; see tests/test_appearance.py for why not entry-wise)."""
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     import diff_gaussian_rasterization as ours
     import wildgaussians_fused as wf
     dev = torch.device("cuda:0")
@@ -126,7 +126,7 @@ def test_fused_render_internal_matches_the_reference_method():
 def test_densification_stats_kernel_matches_the_reference_statements():
     m, Config = wh.import_method()
     if m is None:
-        pytest.skip("reference python package not present (baseline/_ref)")
+        pytest.skip("reference python package not present (oracle/_ref/py)")
     import wildgaussians_fused as wf
     dev = torch.device("cuda:0")
     P = 50_001

@@ -1,5 +1,5 @@
 """CPU tests: the C restatement (oracle/oracle.c) against golden vectors produced by the UNMODIFIED reference
-CUDA rasterizer on a B200 (tests/golden/make_golden.py).  This is what pins the oracle (SURVEY.md 8c)."""
+CUDA rasterizer on a GPU (tests/golden/make_golden.py).  This is what pins the oracle (SURVEY.md 8c)."""
 import numpy as np
 import pytest
 

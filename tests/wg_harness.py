@@ -2,8 +2,8 @@
 
 ``GaussianModel._render_internal`` (method.py:1479-1632) is the caller of the hot path: it builds the camera matrices,
 evaluates the appearance MLP + SH colours in PyTorch and calls ``GaussianRasterizer`` two (or three) times per step.
-This module imports that file as shipped (from ``baseline/_ref``, the pip ``--target`` install of /root/reference made
-by ``__graft_entry__.build()``; or from /root/reference itself where it exists), stubs its three third-party imports
+This module imports that file as shipped (from ``oracle/_ref/py``, the copy of the reference's package made by
+``__graft_entry__.build()`` where the reference checkout can be read), stubs its three third-party imports
 that this path never touches (omegaconf, plyfile, simple_knn), fills a ``GaussianModel`` with a seeded synthetic
 cloud and executes one train-step-like forward + backward:
 
@@ -24,7 +24,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CANDIDATES = [os.path.join(ROOT, "baseline", "_ref"), "/root/reference"]
+CANDIDATES = [os.path.join(ROOT, "oracle", "_ref", "py")]
 
 
 def reference_root():

@@ -2,7 +2,7 @@
 vs the CPU oracle, stage by stage, plus A/B timings.  Not part of the product; the pytest parity tests in
 tests/test_gpu_parity.py are the gate, this prints the detail needed to debug a mismatch.
 
-usage: python tools/gpu_compare.py [--cases small|all] [--time C2,C3] [--out gpurun_out/compare.json]
+usage: python tools/gpu_compare.py [--cases small|all] [--time C2,C3] [--out compare.json]
 """
 from __future__ import annotations
 
@@ -164,7 +164,7 @@ def main():
     ap.add_argument("--cases", default="all")
     ap.add_argument("--time", default="")
     ap.add_argument("--extra", default="", help="comma list of P:W:H[:deg] random scenes for the integer parity check")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "compare.json"))
+    ap.add_argument("--out", default="compare.json")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
     print("host:", os.cpu_count(), "cores;", torch.cuda.get_device_name(0))

@@ -1,4 +1,4 @@
-// appearance.cu -- fused per-Gaussian colour op of wild-gaussians on Blackwell tensor cores (SURVEY.md 8f-2).
+// appearance.cu -- fused per-Gaussian colour op of wild-gaussians on Hopper tensor cores (SURVEY.md 8f-2).
 //
 // What it replaces (PyTorch, wildgaussians/method.py): per Gaussian and per step
 //   features = cat(features_dc, features_rest).clamp_max(1)                          method.py:1063-1066,1570
@@ -10,10 +10,10 @@
 // with dir = normalize(means3D - campos) (:1572): about 60 elementwise / GEMM launches and several P x 128 and
 // P x 48 fp32 intermediates per direction (measured: ~55 ms of a 61 ms train step at P = 3 M).
 //
-// Design: ONE kernel per direction.  A CTA owns tiles of 128 Gaussians (thread = Gaussian = accumulator row = TMEM
-// lane).  The three GEMMs of the MLP run on tcgen05.mma (bf16 operands, fp32 accumulation in TMEM, M = 128); the
-// activations never leave the SM: an epilogue reads the accumulator row with tcgen05.ld, applies ReLU, converts to
-// bf16 and writes the next layer's A operand straight into shared memory ("rows16" storage, umma.cuh).  The packed
+// Design: ONE kernel per direction.  A CTA owns tiles of 128 Gaussians and runs as two warpgroups, each issuing the
+// warpgroup MMAs (wgmma, bf16 operands from shared memory, fp32 accumulation in registers, M = 64) for its 64 rows.  The
+// activations never leave the SM: an epilogue takes the accumulator fragment, applies ReLU, converts to bf16 and writes
+// the next layer's A operand straight into shared memory ("rows16" storage, wgmma.cuh).  The packed
 // weights (49 KB) are fetched once per CTA by one bulk asynchronous copy (TMA engine) and stay resident; each
 // tile's 23 KB of SH coefficients arrive by a bulk copy issued at the start of the tile and consumed in its last
 // epilogue.  Biases ride inside the GEMMs: every A operand carries two constant-one columns and the weight images
@@ -24,19 +24,19 @@
 // Backward: recomputes the three layers per tile (cheaper than storing 2 x 128 activations per Gaussian), then runs
 // the data-gradient chain dO -> dZ2 -> dZ1 -> dX and the three weight-gradient GEMMs on the same shared-memory
 // tiles: an activation tile stored once serves as K-major operand (forward, dgrad) and as MN-major operand (wgrad)
-// without a transposed copy.  Weight gradients accumulate in TMEM across all tiles of the CTA and are reduced to
-// HBM once per CTA with 128-bit reductions.
+// without a transposed copy.  Weight gradients accumulate in registers across all tiles of the CTA and are reduced to
+// HBM once per CTA with vector reductions.
 //
 // Numerics: MLP operands are bf16 (fp32 accumulate); everything else fp32.  Colours agree with the fp32 PyTorch
 // path to ~2e-3 absolute (bf16 rounding of a 128-term dot product scaled by 0.01), gradients to ~1e-2 of their
 // largest magnitude; tests/test_appearance.py states the bars.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "sh_math.cuh"
 
 namespace gsr {
 
-using namespace umma;
+using namespace wg;
 
 constexpr int AP_TILE = 128;
 constexpr int AP_NDC = 3, AP_NREST = 45, AP_NGEMB = 24, AP_NAEMB = 32, AP_H = 128, AP_NOUT = 6;
@@ -190,46 +190,47 @@ __device__ __forceinline__ void build_x_row(const ApParams& p, int row, bool val
                                         pack_bf16(x[8 * c + 4], x[8 * c + 5]), pack_bf16(x[8 * c + 6], x[8 * c + 7])));
 }
 
-// accumulator row (128 fp32 columns at TMEM column `col0`) -> ReLU -> bf16 -> chunks 0..15 of `hbuf`
-// (q0, q1): which of the four 32-column quarters this thread converts -- the backward kernel splits a row between two threads
-__device__ __forceinline__ void relu_epilogue(uint32_t tmem_row, uint32_t col0, uint8_t* hbuf, int t, int q0 = 0, int q1 = 4) {
-#pragma unroll 1
-    for (int q = q0; q < q1; ++q) {
-        float v[32];
-        tmem_ld32(tmem_row + col0 + 32 * q, v);
+// ---- accumulator fragments (wgmma.cuh) ------------------------------------------------------------------------------
+// This thread's accumulator rows within the 128-row tile: r0 and r0 + 8 (warpgroup w owns rows 64 w .. 64 w + 63), and
+// its column pair 2c of every 8-column group.
+struct Frag {
+    int r0, c;
+};
+__device__ __forceinline__ Frag frag_of(int tid) { return {64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2), tid & 3}; }
+__device__ __forceinline__ void st_pair(uint8_t* base, int chunk, int row, int c, uint32_t v) {
+    *reinterpret_cast<uint32_t*>(base + (uint32_t)chunk * CHUNK + (uint32_t)row * 16 + (uint32_t)c * 4) = v;
+}
+__device__ __forceinline__ uint32_t ld_pair(const uint8_t* base, int chunk, int row, int c) {
+    return *reinterpret_cast<const uint32_t*>(base + (uint32_t)chunk * CHUNK + (uint32_t)row * 16 + (uint32_t)c * 4);
+}
+
+// 64 x 128 accumulator -> ReLU -> bf16 -> chunks 0..15 of `hbuf` (this thread's rows only)
+__device__ __forceinline__ void relu_epilogue(const float (&d)[64], uint8_t* hbuf, Frag f) {
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const float* w = v + 8 * c;
-            st_chunk(hbuf, 4 * q + c, t,
-                     make_uint4(pack_bf16(fmaxf(w[0], 0.f), fmaxf(w[1], 0.f)), pack_bf16(fmaxf(w[2], 0.f), fmaxf(w[3], 0.f)),
-                                pack_bf16(fmaxf(w[4], 0.f), fmaxf(w[5], 0.f)), pack_bf16(fmaxf(w[6], 0.f), fmaxf(w[7], 0.f))));
-        }
+    for (int j = 0; j < 16; ++j) {
+        st_pair(hbuf, j, f.r0, f.c, pack_bf16(fmaxf(d[4 * j], 0.f), fmaxf(d[4 * j + 1], 0.f)));
+        st_pair(hbuf, j, f.r0 + 8, f.c, pack_bf16(fmaxf(d[4 * j + 2], 0.f), fmaxf(d[4 * j + 3], 0.f)));
     }
 }
 
-// accumulator row * (activation > 0) -> bf16 -> chunks 0..15 of `dzbuf` (ReLU backward; `hbuf` holds the activation)
-__device__ __forceinline__ void relu_bwd_epilogue(uint32_t tmem_row, uint32_t col0, const uint8_t* hbuf, uint8_t* dzbuf, int t,
-                                                  int q0 = 0, int q1 = 4) {
-#pragma unroll 1
-    for (int q = q0; q < q1; ++q) {
-        float v[32];
-        tmem_ld32(tmem_row + col0 + 32 * q, v);
+// a bf16 activation is positive iff its 15 magnitude bits are non-zero and the sign is clear (ReLU output: never negative)
+__device__ __forceinline__ uint32_t relu_mask(uint32_t h, float lo, float hi) {
+    return pack_bf16((h & 0x7FFFu) ? lo : 0.f, (h & 0x7FFF0000u) ? hi : 0.f);
+}
+// 64 x 128 accumulator * (activation > 0) -> bf16 -> chunks 0..15 of `dzbuf` (ReLU backward; `hbuf` holds the activation)
+__device__ __forceinline__ void relu_bwd_epilogue(const float (&d)[64], const uint8_t* hbuf, uint8_t* dzbuf, Frag f) {
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const uint4 h = ld_chunk(hbuf, 4 * q + c, t);
-            const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
-            float* w = v + 8 * c;
-            uint32_t o[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                // a bf16 activation is positive iff its 15 magnitude bits are non-zero and the sign is clear (ReLU output: never negative)
-                const float lo = (hw[j] & 0x7FFFu) ? w[2 * j] : 0.f;
-                const float hi = (hw[j] & 0x7FFF0000u) ? w[2 * j + 1] : 0.f;
-                o[j] = pack_bf16(lo, hi);
-            }
-            st_chunk(dzbuf, 4 * q + c, t, make_uint4(o[0], o[1], o[2], o[3]));
-        }
+    for (int j = 0; j < 16; ++j) {
+        st_pair(dzbuf, j, f.r0, f.c, relu_mask(ld_pair(hbuf, j, f.r0, f.c), d[4 * j], d[4 * j + 1]));
+        st_pair(dzbuf, j, f.r0 + 8, f.c, relu_mask(ld_pair(hbuf, j, f.r0 + 8, f.c), d[4 * j + 2], d[4 * j + 3]));
     }
+}
+
+// columns 0..7 of the layer-3 accumulator -> fp32 rows of `out` ([128][8]), read back per row by the colour stage
+constexpr uint32_t OUT_BYTES = AP_TILE * 8 * 4;
+__device__ __forceinline__ void store_out(const float (&d)[8], float* out, Frag f) {
+    *reinterpret_cast<float2*>(out + f.r0 * 8 + 2 * f.c) = make_float2(d[0], d[1]);
+    *reinterpret_cast<float2*>(out + (f.r0 + 8) * 8 + 2 * f.c) = make_float2(d[2], d[3]);
 }
 
 // the two constant-one columns (+ zero padding) of an H buffer: chunks 16 and 17
@@ -238,59 +239,76 @@ __device__ __forceinline__ void write_const_chunks(uint8_t* hbuf, int t) {
     st_chunk(hbuf, 17, t, make_uint4(0u, 0u, 0u, 0u));
 }
 
-// the three forward GEMMs are issued by thread 0; every thread then waits on `bar`
-#define AP_WAIT(bar, phase)                                             \
-    do {                                                                \
-        if (!mbar_wait(bar, phase)) { if (p.status) atomicExch(p.status, 1); dead = true; } \
-        phase ^= 1u;                                                    \
-        fence_after_sync();                                             \
+// forward GEMMs of warpgroup `w` (its 64 rows of the K-major activation image `act`, all of the weight image `wimg`);
+// each returns with the accumulator complete
+template <int KSTEPS>
+__device__ __forceinline__ void gemm_n128(float (&d)[64], const uint8_t* act, const uint8_t* wimg, int w) {
+    fence_regs(d);
+    fence();
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) mma_n128<0, 0>(d, desc_k(act + w * 1024, k, AP_TILE), desc_k(wimg, k, AP_H), k > 0);
+    commit_group();
+    wait_all();
+    fence_regs(d);
+}
+__device__ __forceinline__ void gemm_n16(float (&d)[8], const uint8_t* act, const uint8_t* w3p, int w) {
+    fence_regs(d);
+    fence();
+#pragma unroll
+    for (int k = 0; k < AP_K2 / 16; ++k) mma_n16<0, 0>(d, desc_k(act + w * 1024, k, AP_TILE), desc_k(w3p, k, AP_N3), k > 0);
+    commit_group();
+    wait_all();
+    fence_regs(d);
+}
+
+#define AP_FAIL()                                  \
+    do {                                           \
+        if (p.status) atomicExch(p.status, 1);     \
+        dead = true;                               \
     } while (0)
 
 // =====================================================================================================================
 // forward
 // =====================================================================================================================
-constexpr uint32_t FWD_SMEM = BLOB_BYTES + ACT_BYTES + REST_BYTES + 64;
-constexpr int FWD_TMEM_COLS = 256;     // scratch accumulator 128 + layer-3 accumulator 16, power of two
+constexpr uint32_t FWD_SMEM = BLOB_BYTES + ACT_BYTES + REST_BYTES + OUT_BYTES + 64;
 
-// 256 threads per CTA: thread (t, half) = row t, column half `half` of the two wide epilogues (the halves of a row sit in warps
-// w and w + 4, which address the same TMEM lanes); the input row and the colour epilogue are done by half 0.  With two
-// resident CTAs that is 16 warps per SM to hide the tcgen05.ld / shared-memory latency (ncu at 8 warps: 31 % issue-active,
-// long-scoreboard bound).
+// 256 threads = two warpgroups: warpgroup w runs the three GEMMs and their epilogues for rows 64 w .. 64 w + 63 of the tile
+// (wgmma M = 64) and only synchronises with itself between layers; the input row and the colour epilogue of row t are done
+// by thread t < 128.  Two resident CTAs per SM (111 KB of shared memory each) keep 16 warps per SM.
 constexpr int FWD_THREADS = 2 * AP_TILE;
 __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __grid_constant__ ApParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* s_blob = smem;
     uint8_t* s_act = smem + BLOB_BYTES;
     float* s_rest = reinterpret_cast<float*>(smem + BLOB_BYTES + ACT_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BLOB_BYTES + ACT_BYTES + REST_BYTES);   // 0: mma, 1: loads, 2: weights
-    __shared__ uint32_t s_tmem;
-    const int tid = threadIdx.x, t = tid & (AP_TILE - 1), half = tid >> 7, warp = tid >> 5;
-    const bool h0 = half == 0;
-    const int q0 = 2 * half, q1 = 2 * half + 2;
+    float* s_out = reinterpret_cast<float*>(smem + BLOB_BYTES + ACT_BYTES + REST_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BLOB_BYTES + ACT_BYTES + REST_BYTES + OUT_BYTES);   // 0: loads, 1: weights
+    const int tid = threadIdx.x, t = tid & (AP_TILE - 1), w = tid >> 7;
+    const bool h0 = w == 0;
+    const Frag f = frag_of(tid);
 
     if (tid == 0) {
-        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_init(&bars[2], 1);
+        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
         mbar_init_fence();
     }
-    if (warp == 0) tmem_alloc<FWD_TMEM_COLS>(&s_tmem);
     if (h0) write_const_chunks(s_act, t);
     fence_async_smem();
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
     if (tid == 0) {
-        mbar_expect_tx(&bars[2], BLOB_BYTES);
-        bulk_g2s(s_blob, p.blob, BLOB_BYTES, &bars[2]);
+        mbar_expect_tx(&bars[1], BLOB_BYTES);
+        bulk_g2s(s_blob, p.blob, BLOB_BYTES, &bars[1]);
     }
-    const uint32_t tmem = s_tmem;
-    const uint32_t tmem_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
     const uint8_t* w1p = s_blob;
     const uint8_t* w2p = s_blob + W1P_BYTES;
     const uint8_t* w3p = w2p + W2P_BYTES;
-    constexpr uint32_t ID_N128 = instr_desc_bf16(128, 0, 0), ID_N16 = instr_desc_bf16(16, 0, 0);
-    uint32_t ph_mma = 0, ph_ld = 0;
+    float acc[64], acc3[8];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc3[i] = 0.f;
+    uint32_t ph_ld = 0;
     bool dead = false;
-    if (!mbar_wait(&bars[2], 0)) { if (p.status) atomicExch(p.status, 1); dead = true; }
+    if (!mbar_wait(&bars[1], 0)) AP_FAIL();
 
     for (int tile = blockIdx.x; tile < p.num_tiles && !dead; tile += gridDim.x) {
         const int row0 = tile * AP_TILE, row = row0 + t;
@@ -299,8 +317,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __
         const bool bulk = rows == AP_TILE;           // whole tiles: one 23 KB bulk copy; the ragged last tile: plain loads
         if (bulk) {
             if (tid == 0) {
-                mbar_expect_tx(&bars[1], REST_BYTES);
-                bulk_g2s(s_rest, p.rest + (size_t)row0 * AP_NREST, REST_BYTES, &bars[1]);
+                mbar_expect_tx(&bars[0], REST_BYTES);
+                bulk_g2s(s_rest, p.rest + (size_t)row0 * AP_NREST, REST_BYTES, &bars[0]);
             }
         } else {
             for (int i = tid; i < rows * AP_NREST; i += FWD_THREADS) s_rest[i] = p.rest[(size_t)row0 * AP_NREST + i];
@@ -309,41 +327,25 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __
         in.dc[0] = in.dc[1] = in.dc[2] = 0.f; in.dir = {0.f, 0.f, 1.f}; in.inv_norm = 0.f;
         if (h0) build_x_row(p, row, valid, t, s_act, in);
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K1 / 16; ++k) mma_bf16(tmem, desc_k(s_act, k, AP_TILE), desc_k(w1p, k, AP_H), ID_N128, k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_epilogue(tmem_row, 0, s_act, t, q0, q1);
+        // a warpgroup's GEMM reads only its own 64 rows of the activation image, which only its own threads overwrite
+        gemm_n128<AP_K1 / 16>(acc, s_act, w1p, w);
+        relu_epilogue(acc, s_act, f);
         fence_async_smem();
-        fence_before_sync();
-        __syncthreads();
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K2 / 16; ++k) mma_bf16(tmem, desc_k(s_act, k, AP_TILE), desc_k(w2p, k, AP_H), ID_N128, k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_epilogue(tmem_row, 0, s_act, t, q0, q1);
+        warpgroup_sync(w);
+        gemm_n128<AP_K2 / 16>(acc, s_act, w2p, w);
+        relu_epilogue(acc, s_act, f);
         fence_async_smem();
-        fence_before_sync();
+        warpgroup_sync(w);
+        gemm_n16(acc3, s_act, w3p, w);
+        store_out(acc3, s_out, f);
         __syncthreads();
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K2 / 16; ++k) mma_bf16(tmem + 128, desc_k(s_act, k, AP_TILE), desc_k(w3p, k, AP_N3), ID_N16, k > 0);
-            commit(&bars[0]);
+        if (bulk) {
+            if (!mbar_wait(&bars[0], ph_ld)) AP_FAIL();
+            ph_ld ^= 1u;
         }
-        AP_WAIT(&bars[0], ph_mma);
-        float o[16];
-        if (h0) tmem_ld16(tmem_row + 128, o);
-        if (bulk) { if (!mbar_wait(&bars[1], ph_ld)) { if (p.status) atomicExch(p.status, 1); dead = true; } ph_ld ^= 1u; }
         if (valid) {
+            const float* o = s_out + t * 8;
             float b[16];
             sh_basis(p.deg, in.dir.x, in.dir.y, in.dir.z, b);
             const float* fr = s_rest + t * AP_NREST;
@@ -355,9 +357,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __
                 float r = b[0] * f0, s = b[0] * fminf(fmaf(f0, mul, off), 1.0f);
 #pragma unroll
                 for (int k = 1; k < 16; ++k) {
-                    const float f = fminf(fr[3 * (k - 1) + c], 1.0f);
-                    r = fmaf(b[k], f, r);
-                    s = fmaf(b[k], fminf(f * mul, 1.0f), s);
+                    const float fv = fminf(fr[3 * (k - 1) + c], 1.0f);
+                    r = fmaf(b[k], fv, r);
+                    s = fmaf(b[k], fminf(fv * mul, 1.0f), s);
                 }
                 sr[c] = fmaxf(r + 0.5f, 0.f);
                 st[c] = fmaxf(s + 0.5f, 0.f);
@@ -369,13 +371,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __
             }
         }
         fence_async_smem();       // generic reads of s_rest / s_act are ordered before the next tile's bulk copy into them
-        fence_before_sync();
-        __syncthreads();          // s_rest and s_act are free for the next tile
-        fence_after_sync();
+        __syncthreads();          // s_rest, s_act and s_out are free for the next tile
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_free<FWD_TMEM_COLS>(tmem);
 }
 
 // =====================================================================================================================
@@ -384,16 +381,29 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_fwd_kernel(const __
 constexpr uint32_t BX_BYTES = (AP_K1 / 8) * CHUNK;        //  8192
 constexpr uint32_t BDZ_BYTES = (AP_H / 8) * CHUNK;        // 32768
 constexpr uint32_t BDO_BYTES = (AP_N3 / 8) * CHUNK;       //  4096
-constexpr uint32_t BWD_SMEM = BLOB_BYTES + BX_BYTES + 2 * ACT_BYTES + BDZ_BYTES + BDO_BYTES + REST_BYTES + 128;
-// TMEM columns: scratch 0..127 | layer-3 128..143 | dX 160..191 | acc dW2p 192..335 | acc dW1p 336..367 | acc dW3pT 368..383
-constexpr uint32_t TC_D3 = 128, TC_DX = 160, TC_W2 = 192, TC_W1 = 336, TC_W3 = 368;
+constexpr int DX_LD = 36;                                 // fp32 row stride of the dX tile: conflict-free pair stores
+constexpr uint32_t BDX_BYTES = AP_TILE * DX_LD * 4;       // 18432
+constexpr uint32_t BWD_SMEM = BLOB_BYTES + BX_BYTES + 2 * ACT_BYTES + BDZ_BYTES + BDO_BYTES + REST_BYTES + OUT_BYTES + BDX_BYTES + 128;
 
-// 256 threads: thread (t, half) -- row t of the tile, column half `half` of the wide epilogues.  The two halves of a row sit in
-// warps w and w + 4, which address the same 32 TMEM lanes (lane base = 32 * (warp % 4)); eight warps per SM instead of four
-// hide the tcgen05.ld / shared-memory latency of the four 128-column epilogues.  Per-row work that cannot be split (input row,
-// colour stage, dX) is done by half 0.
+// red.global.add.v2 of a weight-gradient accumulator fragment into the fp32 image `g` (row stride ld)
+template <int R>
+__device__ __forceinline__ void flush_frag(const float (&d)[R], float* g, int ld, Frag f) {
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+        float* a = g + (size_t)f.r0 * ld + 8 * j + 2 * f.c;
+        float* b = a + (size_t)8 * ld;
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(a), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(b), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+    }
+}
+
+// 256 threads = two warpgroups.  Data-gradient GEMMs (M = Gaussians): warpgroup w takes rows 64 w .. 64 w + 63 of the tile.
+// Weight-gradient GEMMs (K = the 128 Gaussians of the tile): warpgroup w takes rows 64 w .. 64 w + 63 of each gradient
+// image, whose accumulators stay in registers across all tiles of the CTA (dW2p 72 + dW1p 16 + dW3pT 8 per thread) and
+// are reduced to HBM once per CTA.  Per-row work that cannot be split (input row, colour stage, dX) is done by thread
+// t < 128.  One CTA per SM (209 KB of shared memory).
 constexpr int BWD_THREADS = 2 * AP_TILE;
-__global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __grid_constant__ ApParams p) {
+__global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __grid_constant__ ApParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* s_blob = smem;
     uint8_t* s_x = s_blob + BLOB_BYTES;
@@ -402,43 +412,47 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
     uint8_t* s_dz = s_h2 + ACT_BYTES;
     uint8_t* s_do = s_dz + BDZ_BYTES;
     float* s_rest = reinterpret_cast<float*>(s_do + BDO_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_rest) + REST_BYTES);
+    float* s_out = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(s_rest) + REST_BYTES);
+    float* s_dx = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(s_out) + OUT_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_dx) + BDX_BYTES);
     float* s_db3 = reinterpret_cast<float*>(bars + 4);       // [8]
-    __shared__ uint32_t s_tmem;
-    const int tid = threadIdx.x, t = tid & (AP_TILE - 1), half = tid >> 7, warp = tid >> 5, lane = tid & 31;
-    const bool h0 = half == 0;
-    const int q0 = 2 * half, q1 = 2 * half + 2;
+    const int tid = threadIdx.x, t = tid & (AP_TILE - 1), w = tid >> 7, lane = tid & 31;
+    const bool h0 = w == 0;
+    const Frag f = frag_of(tid);
+    constexpr uint32_t MN_HALF = 8 * CHUNK;                   // warpgroup w's 64 M rows of an MN-major operand
 
     if (tid == 0) {
-        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_init(&bars[2], 1);
+        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
         mbar_init_fence();
     }
     if (tid < 8) s_db3[tid] = 0.f;
-    if (warp == 0) tmem_alloc<512>(&s_tmem);
     if (h0) {
         write_const_chunks(s_h1, t);
         write_const_chunks(s_h2, t);
         st_chunk(s_do, 1, t, make_uint4(0u, 0u, 0u, 0u));
     }
     fence_async_smem();
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
     if (tid == 0) {
-        mbar_expect_tx(&bars[2], BLOB_BYTES);
-        bulk_g2s(s_blob, p.blob, BLOB_BYTES, &bars[2]);
+        mbar_expect_tx(&bars[1], BLOB_BYTES);
+        bulk_g2s(s_blob, p.blob, BLOB_BYTES, &bars[1]);
     }
-    const uint32_t tmem = s_tmem;
-    const uint32_t tmem_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
     const uint8_t* w1p = s_blob;
     const uint8_t* w2p = s_blob + W1P_BYTES;
     const uint8_t* w3p = w2p + W2P_BYTES;
-    constexpr uint32_t ID_F128 = instr_desc_bf16(128, 0, 0), ID_F16 = instr_desc_bf16(16, 0, 0);
-    constexpr uint32_t ID_DG128 = instr_desc_bf16(128, 0, 1), ID_DG32 = instr_desc_bf16(32, 0, 1);        // dgrad: A K-major, B MN-major
-    constexpr uint32_t ID_WG144 = instr_desc_bf16(144, 1, 1), ID_WG32 = instr_desc_bf16(32, 1, 1), ID_WG16 = instr_desc_bf16(16, 1, 1);
-    uint32_t ph_mma = 0, ph_ld = 0;
+    float gw2[72], gw1[16], gw3[8];           // weight-gradient accumulators: start at zero, always accumulate
+    float acc[64], acc3[8], accx[16];
+#pragma unroll
+    for (int i = 0; i < 72; ++i) gw2[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) { gw1[i] = 0.f; accx[i] = 0.f; }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { gw3[i] = 0.f; acc3[i] = 0.f; }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    uint32_t ph_ld = 0;
     bool dead = false;
-    if (!mbar_wait(&bars[2], 0)) { if (p.status) atomicExch(p.status, 1); dead = true; }
+    if (!mbar_wait(&bars[1], 0)) AP_FAIL();
     int iter = 0;
 
     for (int tile = blockIdx.x; tile < p.num_tiles && !dead; tile += gridDim.x, ++iter) {
@@ -446,11 +460,10 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
         const int rows = min(AP_TILE, p.P - row0);
         const bool valid = h0 && t < rows;
         const bool bulk = rows == AP_TILE;
-        const bool acc = iter > 0;
         if (bulk) {
             if (tid == 0) {
-                mbar_expect_tx(&bars[1], REST_BYTES);
-                bulk_g2s(s_rest, p.rest + (size_t)row0 * AP_NREST, REST_BYTES, &bars[1]);
+                mbar_expect_tx(&bars[0], REST_BYTES);
+                bulk_g2s(s_rest, p.rest + (size_t)row0 * AP_NREST, REST_BYTES, &bars[0]);
             }
         } else {
             for (int i = tid; i < rows * AP_NREST; i += BWD_THREADS) s_rest[i] = p.rest[(size_t)row0 * AP_NREST + i];
@@ -459,46 +472,29 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
         in.dc[0] = in.dc[1] = in.dc[2] = 0.f; in.dir = {0.f, 0.f, 1.f}; in.inv_norm = 0.f;
         if (h0) build_x_row(p, row, valid, t, s_x, in);
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
-        // ---- forward recompute -----------------------------------------------------------------------------------
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K1 / 16; ++k) mma_bf16(tmem, desc_k(s_x, k, AP_TILE), desc_k(w1p, k, AP_H), ID_F128, k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_epilogue(tmem_row, 0, s_h1, t, q0, q1);
+        // ---- forward recompute (per warpgroup, as in the forward kernel) ----------------------------------------------
+        gemm_n128<AP_K1 / 16>(acc, s_x, w1p, w);
+        relu_epilogue(acc, s_h1, f);
         fence_async_smem();
-        fence_before_sync();
-        __syncthreads();
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K2 / 16; ++k) mma_bf16(tmem, desc_k(s_h1, k, AP_TILE), desc_k(w2p, k, AP_H), ID_F128, k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_epilogue(tmem_row, 0, s_h2, t, q0, q1);
+        warpgroup_sync(w);
+        gemm_n128<AP_K2 / 16>(acc, s_h1, w2p, w);
+        relu_epilogue(acc, s_h2, f);
         fence_async_smem();
-        fence_before_sync();
+        warpgroup_sync(w);
+        gemm_n16(acc3, s_h2, w3p, w);
+        store_out(acc3, s_out, f);
         __syncthreads();
-        if (tid == 0) {
-            fence_after_sync();
-#pragma unroll
-            for (int k = 0; k < AP_K2 / 16; ++k) mma_bf16(tmem + TC_D3, desc_k(s_h2, k, AP_TILE), desc_k(w3p, k, AP_N3), ID_F16, k > 0);
-            commit(&bars[0]);
+        if (bulk) {
+            if (!mbar_wait(&bars[0], ph_ld)) AP_FAIL();
+            ph_ld ^= 1u;
         }
-        AP_WAIT(&bars[0], ph_mma);
-        float o[16];
-        if (h0) tmem_ld16(tmem_row + TC_D3, o);
-        if (bulk) { if (!mbar_wait(&bars[1], ph_ld)) { if (p.status) atomicExch(p.status, 1); dead = true; } ph_ld ^= 1u; }
 
         // ---- colour stage backward: dL/d{raw, toned} -> dL/d features, dL/d(offset, mul), dL/d mean ----------------
         float dOut[AP_NOUT] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         float g_dc[3] = {0.f, 0.f, 0.f};          // gradient w.r.t. min(dc, 1) from the colour sums (the MLP path is added later)
         if (valid) {
+            const float* o = s_out + t * 8;
             float b[16], gk[16];
             sh_basis(p.deg, in.dir.x, in.dir.y, in.dir.z, b);
 #pragma unroll
@@ -512,9 +508,9 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
                 float r = b[0] * f0, s = b[0] * fminf(t0p, 1.0f);
 #pragma unroll
                 for (int k = 1; k < 16; ++k) {
-                    const float f = fminf(fr[3 * (k - 1) + c], 1.0f);
-                    r = fmaf(b[k], f, r);
-                    s = fmaf(b[k], fminf(f * mul, 1.0f), s);
+                    const float fv = fminf(fr[3 * (k - 1) + c], 1.0f);
+                    r = fmaf(b[k], fv, r);
+                    s = fmaf(b[k], fminf(fv * mul, 1.0f), s);
                 }
                 // clamp_min(x + 0.5, 0) passes the gradient where x + 0.5 >= 0
                 const float dLr = (p.dL_raw != nullptr && r + 0.5f >= 0.f) ? p.dL_raw[(size_t)row * 3 + c] : 0.f;
@@ -530,11 +526,11 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
 #pragma unroll
                 for (int k = 1; k < 16; ++k) {
                     const float fu = fr[3 * (k - 1) + c];
-                    const float f = fminf(fu, 1.0f);
-                    const float tp = f * mul;
+                    const float fv = fminf(fu, 1.0f);
+                    const float tp = fv * mul;
                     const float dt = (tp <= 1.0f) ? b[k] * dLt : 0.f;
-                    dmul = fmaf(dt, f, dmul);
-                    gk[k] += dLr * f + dLt * fminf(tp, 1.0f);
+                    dmul = fmaf(dt, fv, dmul);
+                    gk[k] += dLr * fv + dLt * fminf(tp, 1.0f);
                     // gradient of features_rest (clamp_max(1) passes it where the raw value <= 1), written in place
                     fr[3 * (k - 1) + c] = (fu <= 1.0f) ? fmaf(dt, mul, b[k] * dLr) : 0.f;
                 }
@@ -559,93 +555,76 @@ __global__ void __launch_bounds__(BWD_THREADS) appearance_bwd_kernel(const __gri
             }
         }
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
         // coalesced copy-out of the tile's features_rest gradients (they replaced the features in s_rest)
         for (int i = tid; i < rows * AP_NREST; i += BWD_THREADS) p.g_rest[(size_t)row0 * AP_NREST + i] = s_rest[i];
         // ---- layer 3 backward --------------------------------------------------------------------------------------
-        if (tid == 0) {
-            fence_after_sync();
-            // dH2 = dO . W3           A: dO K-major (K = 16 outputs), B: W3p as MN-major (N = 128 inputs)
-            mma_bf16(tmem, desc_k(s_do, 0, AP_TILE), desc_mn(w3p, 0, AP_N3), ID_DG128, false);
-            // dW3p^T[128 in][16 out] += H2^T . dO      both MN-major, K = the 128 Gaussians of the tile
+        fence_regs(acc); fence_regs(gw3);
+        fence();
+        // dH2 = dO . W3           A: dO K-major (K = 16 outputs), B: W3p as MN-major (N = 128 inputs)
+        mma_n128<0, 1>(acc, desc_k(s_do + w * 1024, 0, AP_TILE), desc_mn(w3p, 0, AP_N3), false);
+        // dW3p^T[128 in][16 out] += H2^T . dO      both MN-major, K = the 128 Gaussians of the tile
 #pragma unroll
-            for (int k = 0; k < AP_TILE / 16; ++k)
-                mma_bf16(tmem + TC_W3, desc_mn(s_h2, k, AP_TILE), desc_mn(s_do, k, AP_TILE), ID_WG16, acc || k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_bwd_epilogue(tmem_row, 0, s_h2, s_dz, t, q0, q1);
+        for (int k = 0; k < AP_TILE / 16; ++k) mma_n16<1, 1>(gw3, desc_mn(s_h2 + w * MN_HALF, k, AP_TILE), desc_mn(s_do, k, AP_TILE), true);
+        commit_group();
+        wait_all();
+        fence_regs(acc); fence_regs(gw3);
+        relu_bwd_epilogue(acc, s_h2, s_dz, f);
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
         // ---- layer 2 backward --------------------------------------------------------------------------------------
-        if (tid == 0) {
-            fence_after_sync();
-            // dW2p[128 out][144 in] += dZ2^T . H1p   (column 128 of H1p is the constant one: bias gradient)
+        fence_regs(acc); fence_regs(gw2);
+        fence();
+        // dW2p[128 out][144 in] += dZ2^T . H1p   (column 128 of H1p is the constant one: bias gradient)
 #pragma unroll
-            for (int k = 0; k < AP_TILE / 16; ++k)
-                mma_bf16(tmem + TC_W2, desc_mn(s_dz, k, AP_TILE), desc_mn(s_h1, k, AP_TILE), ID_WG144, acc || k > 0);
-            // dH1 = dZ2 . W2          A: dZ2 K-major (K = 128 outputs), B: W2p MN-major (N = 128 inputs)
+        for (int k = 0; k < AP_TILE / 16; ++k) mma_n144<1, 1>(gw2, desc_mn(s_dz + w * MN_HALF, k, AP_TILE), desc_mn(s_h1, k, AP_TILE), true);
+        // dH1 = dZ2 . W2          A: dZ2 K-major (K = 128 outputs), B: W2p MN-major (N = 128 inputs)
 #pragma unroll
-            for (int k = 0; k < AP_H / 16; ++k) mma_bf16(tmem, desc_k(s_dz, k, AP_TILE), desc_mn(w2p, k, AP_H), ID_DG128, k > 0);
-            commit(&bars[0]);
-        }
-        AP_WAIT(&bars[0], ph_mma);
-        relu_bwd_epilogue(tmem_row, 0, s_h1, s_dz, t, q0, q1);
+        for (int k = 0; k < AP_H / 16; ++k) mma_n128<0, 1>(acc, desc_k(s_dz + w * 1024, k, AP_TILE), desc_mn(w2p, k, AP_H), k > 0);
+        commit_group();
+        wait_all();
+        fence_regs(acc); fence_regs(gw2);
+        __syncthreads();          // the other warpgroup's weight-gradient GEMM reads every row of s_dz
+        relu_bwd_epilogue(acc, s_h1, s_dz, f);
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
         // ---- layer 1 backward --------------------------------------------------------------------------------------
-        if (tid == 0) {
-            fence_after_sync();
+        fence_regs(accx); fence_regs(gw1);
+        fence();
 #pragma unroll
-            for (int k = 0; k < AP_TILE / 16; ++k)
-                mma_bf16(tmem + TC_W1, desc_mn(s_dz, k, AP_TILE), desc_mn(s_x, k, AP_TILE), ID_WG32, acc || k > 0);
+        for (int k = 0; k < AP_TILE / 16; ++k) mma_n32<1, 1>(gw1, desc_mn(s_dz + w * MN_HALF, k, AP_TILE), desc_mn(s_x, k, AP_TILE), true);
 #pragma unroll
-            for (int k = 0; k < AP_H / 16; ++k) mma_bf16(tmem + TC_DX, desc_k(s_dz, k, AP_TILE), desc_mn(w1p, k, AP_H), ID_DG32, k > 0);
-            commit(&bars[0]);
+        for (int k = 0; k < AP_H / 16; ++k) mma_n32<0, 1>(accx, desc_k(s_dz + w * 1024, k, AP_TILE), desc_mn(w1p, k, AP_H), k > 0);
+        commit_group();
+        wait_all();
+        fence_regs(accx); fence_regs(gw1);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            *reinterpret_cast<float2*>(s_dx + f.r0 * DX_LD + 8 * j + 2 * f.c) = make_float2(accx[4 * j], accx[4 * j + 1]);
+            *reinterpret_cast<float2*>(s_dx + (f.r0 + 8) * DX_LD + 8 * j + 2 * f.c) = make_float2(accx[4 * j + 2], accx[4 * j + 3]);
         }
-        AP_WAIT(&bars[0], ph_mma);
-        if (h0) {
-            float dx[32];
-            tmem_ld32(tmem_row + TC_DX, dx);
-            if (valid) {
-#pragma unroll
-                for (int c = 0; c < 3; ++c)      // x[c] = min(dc, 1): both paths pass where dc <= 1
-                    p.g_dc[(size_t)row * 3 + c] = (in.dc[c] <= 1.0f) ? g_dc[c] + dx[c] : 0.f;
-                float4* gg = reinterpret_cast<float4*>(p.g_gemb + (size_t)row * AP_NGEMB);
-#pragma unroll
-                for (int i = 0; i < AP_NGEMB / 4; ++i) gg[i] = make_float4(dx[3 + 4 * i], dx[4 + 4 * i], dx[5 + 4 * i], dx[6 + 4 * i]);
-            }
-        }
-        fence_before_sync();
         __syncthreads();
-        fence_after_sync();
+        if (valid) {
+            const float* dx = s_dx + t * DX_LD;
+#pragma unroll
+            for (int c = 0; c < 3; ++c)      // x[c] = min(dc, 1): both paths pass where dc <= 1
+                p.g_dc[(size_t)row * 3 + c] = (in.dc[c] <= 1.0f) ? g_dc[c] + dx[c] : 0.f;
+            float4* gg = reinterpret_cast<float4*>(p.g_gemb + (size_t)row * AP_NGEMB);
+#pragma unroll
+            for (int i = 0; i < AP_NGEMB / 4; ++i) gg[i] = make_float4(dx[3 + 4 * i], dx[4 + 4 * i], dx[5 + 4 * i], dx[6 + 4 * i]);
+        }
+        fence_async_smem();
+        __syncthreads();
     }
 
     // ---- reduce the CTA's weight-gradient accumulators to HBM ---------------------------------------------------------
     if (iter > 0 && !dead) {
         float* g = p.g_pack;
-        auto flush = [&](uint32_t col0, int ncols, size_t base, int ld) {
-            for (int c0 = 16 * half; c0 < ncols; c0 += 32) {      // the two halves of a row take alternate 16-column groups
-                float v[16];
-                tmem_ld16(tmem_row + col0 + c0, v);
-                float* dst = g + base + (size_t)t * ld + c0;
-#pragma unroll
-                for (int j = 0; j < 16; j += 4)
-                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(v[j]), "f"(v[j + 1]), "f"(v[j + 2]),
-                                 "f"(v[j + 3]) : "memory");
-            }
-        };
-        flush(TC_W2, AP_K2, GW2P, AP_K2);
-        flush(TC_W1, AP_K1, GW1P, AP_K1);
-        flush(TC_W3, AP_N3, GW3P, AP_N3);
+        flush_frag(gw2, g + GW2P, AP_K2, f);
+        flush_frag(gw1, g + GW1P, AP_K1, f);
+        flush_frag(gw3, g + GW3P, AP_N3, f);
         if (tid < AP_NOUT) atomicAdd(g + GB3 + tid, s_db3[tid]);
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_free<512>(tmem);
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------
@@ -654,7 +633,7 @@ static int ap_num_sms() {
     if (n == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of libgsrast (sm_100a Gaussian-splat rasterizer).
+// common.cuh -- shared declarations of libgsrast (sm_90a Gaussian-splat rasterizer).
 // Internal header: the public boundary is include/gsrast.h.
 #pragma once
 #include <cuda_runtime.h>

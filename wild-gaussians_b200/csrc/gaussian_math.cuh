@@ -70,13 +70,17 @@ __device__ __forceinline__ float4 xform_point_4x4(const float3& p, const float* 
     return t;
 }
 
-// rotation (raw quaternion r,x,y,z -- NOT normalised, note N5) as column-major matrix
+// rotation (raw quaternion r,x,y,z -- NOT normalised, note N5) as column-major matrix.
+// The reference's contraction is written out (oracle/oracle.c quat_to_R): xz, rx, rz, yy, zz are rounded products,
+// r*y, y*z, x*y, x*x are fused into the add / sub.  Which products ptxas fuses here depends on the target
+// architecture, so the pattern is not left to the compiler.
 __device__ __forceinline__ Mat3 quat_to_mat(const float4 q) {
     const float r = q.x, x = q.y, y = q.z, z = q.w;
+    const float xz = __fmul_rn(x, z), rx = __fmul_rn(r, x), rz = __fmul_rn(r, z), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
     return mat3_cols(
-        1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y),
-        2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x),
-        2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y));
+        1.f - 2.f * __fadd_rn(yy, zz), 2.f * __fmaf_rn(x, y, -rz), 2.f * __fmaf_rn(r, y, xz),
+        2.f * __fmaf_rn(x, y, rz), 1.f - 2.f * __fmaf_rn(x, x, zz), 2.f * __fmaf_rn(y, z, -rx),
+        2.f * __fmaf_rn(-r, y, xz), 2.f * __fmaf_rn(y, z, rx), 1.f - 2.f * __fmaf_rn(x, x, yy));
 }
 
 // world-space covariance from scale and rotation; upper triangle in cov[6]

@@ -255,7 +255,7 @@ extern "C" int gsr_knn_mean_dist2(int P, const float* points, float* mean_dist2,
     // bounding box (ordered-int encoding: min slots start at +max, max slots at -max)
     const int init[6] = {0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, (int)0x80800000, (int)0x80800000, (int)0x80800000};
     GSR_CUDA(cudaMemcpyAsync(k.bbox, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    knn_bbox_kernel<<<min(grid, 148 * 8), KNN_THREADS, 0, s>>>(P, points, k.bbox);
+    knn_bbox_kernel<<<min(grid, 132 * 8), KNN_THREADS, 0, s>>>(P, points, k.bbox);
     knn_morton_kernel<<<grid, KNN_THREADS, 0, s>>>(P, points, k.bbox, k.key_a, k.key_hi, k.val_a);
     count_launches(2);
     GSR_CUDA(cudaGetLastError());

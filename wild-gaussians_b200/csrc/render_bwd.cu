@@ -342,11 +342,9 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
     }
 }
 
-// ---- packed variant: 2 pixels per lane, their arithmetic paired in Blackwell's 2-wide fp32 instructions ------
-// sm_100 adds FADD2 / FMUL2 / FFMA2 (PTX add/mul/fma.rn.f32x2): one issue slot performs the operation on a pair of
-// fp32 values held in an aligned register pair.  The composite kernels are bound by instruction issue (ncu: 85 %
-// issue-active, < 3 % DRAM), so pairing the two pixels of a lane halves the issue cost of the floating-point part.
-// IEEE rounding per element is that of the scalar instruction: the expression shapes that decide which pairs blend
+// ---- packed variant: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2, render_common.cuh) ----
+// Both pixels of a lane share every per-Gaussian operand load and the loop control, and the fused epilogues (peer
+// reduction, touched marks) exist in this kernel only.  IEEE rounding per element is that of the scalar instruction: the expression shapes that decide which pairs blend
 // (power, alpha; forward.cu:353-368) are the same trees as in the scalar kernel, fused exactly where nvcc fuses them.
 // Per-Gaussian operands are staged in shared memory already duplicated ({x, x, y, y} ...) so that one LDS.128 yields
 // two ready-made broadcast pairs and no register moves are needed.
@@ -477,13 +475,13 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
 
                 // power = -0.5 (A dx dx + C dy dy) - B dx dy, contracted as nvcc contracts the scalar expression:
                 //   s = fma(dx, A dx, (C dy) dy);  power = fma(s, -0.5, -((B dx) dy))      (checked against the SASS)
-                const float2 dx = __fadd2_rn(lo2(xy), npx), dy = __fadd2_rn(hi2(xy), npy);
-                const float2 t1 = __fmul2_rn(lo2(ac), dx);
-                const float2 t3 = __fmul2_rn(dy, __fmul2_rn(hi2(ac), dy));
-                const float2 un = __fmul2_rn(dy, __fmul2_rn(lo2(bo), dx));       // -(B dx) dy
-                const float2 power = __ffma2_rn(__ffma2_rn(dx, t1, t3), mhalf, un);
+                const float2 dx = add2(lo2(xy), npx), dy = add2(hi2(xy), npy);
+                const float2 t1 = mul2(lo2(ac), dx);
+                const float2 t3 = mul2(dy, mul2(hi2(ac), dy));
+                const float2 un = mul2(dy, mul2(lo2(bo), dx));       // -(B dx) dy
+                const float2 power = fma2(fma2(dx, t1, t3), mhalf, un);
                 const float g0 = expf(power.x), g1 = expf(power.y);
-                const float2 oG = __fmul2_rn(hi2(bo), make_float2(g0, g1));
+                const float2 oG = mul2(hi2(bo), make_float2(g0, g1));
                 const float a0 = min(0.99f, oG.x), a1 = min(0.99f, oG.y);
                 const bool act0 = pos < last_contributor[0] && !(power.x > 0.0f) && !(a0 < 1.0f / 255.0f);
                 const bool act1 = pos < last_contributor[1] && !(power.y > 0.0f) && !(a1 < 1.0f / 255.0f);
@@ -493,24 +491,24 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
                 const float2 alpha = make_float2(act0 ? a0 : 0.f, act1 ? a1 : 0.f);
 
                 const float4 rg = R.rg, bk = R.bk;
-                const float2 oma = __fadd2_rn(one, make_float2(-alpha.x, -alpha.y));
+                const float2 oma = add2(one, make_float2(-alpha.x, -alpha.y));
                 const float2 inv = make_float2(rcp_approx(oma.x), rcp_approx(oma.y));
-                T = __fmul2_rn(T, inv);
-                const float2 aT = __fmul2_rn(alpha, T);
-                rdot = __ffma2_rn(last_alpha, __fadd2_rn(last_cd, make_float2(-rdot.x, -rdot.y)), rdot);
-                const float2 cd = __ffma2_rn(lo2(bk), dL2, __ffma2_rn(hi2(rg), dL1, __fmul2_rn(lo2(rg), dL0)));
+                T = mul2(T, inv);
+                const float2 aT = mul2(alpha, T);
+                rdot = fma2(last_alpha, add2(last_cd, make_float2(-rdot.x, -rdot.y)), rdot);
+                const float2 cd = fma2(lo2(bk), dL2, fma2(hi2(rg), dL1, mul2(lo2(rg), dL0)));
                 last_cd = cd;
                 last_alpha = alpha;
-                const float2 dL_dalpha = __ffma2_rn(__fadd2_rn(cd, make_float2(-rdot.x, -rdot.y)), T, __fmul2_rn(Tb, inv));
-                const float2 wgt = __fmul2_rn(G, dL_dalpha);
-                const float2 wx = __fmul2_rn(wgt, dx), wy = __fmul2_rn(wgt, dy);
+                const float2 dL_dalpha = fma2(add2(cd, make_float2(-rdot.x, -rdot.y)), T, mul2(Tb, inv));
+                const float2 wgt = mul2(G, dL_dalpha);
+                const float2 wx = mul2(wgt, dx), wy = mul2(wgt, dy);
                 // t1 = A wx + B wy, t2 = C wy + B wx  (lo2(bo) holds -B: the sign disappears under |.|)
-                const float2 q1 = __ffma2_rn(lo2(bo), wy, make_float2(-0.f, -0.f));   // -B wy
-                const float2 u1 = __ffma2_rn(lo2(ac), wx, make_float2(-q1.x, -q1.y));
-                const float2 q2 = __fmul2_rn(lo2(bo), wx);                             // -B wx
-                const float2 u2 = __ffma2_rn(hi2(ac), wy, make_float2(-q2.x, -q2.y));
-                const float2 mxx = __fmul2_rn(wx, dx), mxy = __fmul2_rn(wx, dy), myy = __fmul2_rn(wy, dy);
-                const float2 c0 = __fmul2_rn(aT, dL0), c1 = __fmul2_rn(aT, dL1), c2 = __fmul2_rn(aT, dL2);
+                const float2 q1 = fma2(lo2(bo), wy, make_float2(-0.f, -0.f));   // -B wy
+                const float2 u1 = fma2(lo2(ac), wx, make_float2(-q1.x, -q1.y));
+                const float2 q2 = mul2(lo2(bo), wx);                             // -B wx
+                const float2 u2 = fma2(hi2(ac), wy, make_float2(-q2.x, -q2.y));
+                const float2 mxx = mul2(wx, dx), mxy = mul2(wx, dy), myy = mul2(wy, dy);
+                const float2 c0 = mul2(aT, dL0), c1 = mul2(aT, dL1), c2 = mul2(aT, dL2);
                 float v[10];
                 v[0] = wx.x + wx.y;
                 v[1] = wy.x + wy.y;

@@ -20,6 +20,15 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
 }
 
+// Pair arithmetic of the packed composite kernels: each element is rounded exactly like the scalar instruction and
+// never contracted, so a pair gives the scalar kernel's bits.  sm_90 has no 2-wide fp32 instructions; the pairing
+// keeps the packed kernels' staging (one LDS.128 = two ready-made broadcast pairs) and their fused epilogues.
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // Thread -> pixel mapping inside a 16x16 tile.  A thread owns PPT pixels (1, 2 or 4) arranged PX x PY,
 // a warp owns a compact block of (8 PX) x (4 PY) pixels (the reference: one pixel per thread, a warp =
 // a 16x2 strip).  Per-pixel results do not depend on the mapping.  More pixels per thread amortise the

@@ -193,9 +193,8 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_fwd_kernel(cons
     }
 }
 
-// ---- packed variant: 2 pixels per lane, their arithmetic paired in FADD2 / FMUL2 / FFMA2 ---------------------
-// (see render_bwd.cu for the rationale: the composite is issue-bound; sm_100's 2-wide fp32 instructions halve the
-// issue cost of everything that is not expf / compare / select.)  Every element of a pair goes through the same
+// ---- packed variant: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2) ----------------
+// (see render_bwd.cu: both pixels of a lane share every per-Gaussian operand load and the loop control.)  Every element of a pair goes through the same
 // IEEE operations, in the same order, as the scalar kernel above -- power = fma(fma(dx, A dx, (C dy) dy), -0.5,
 // -((B dx) dy)), alpha = min(0.99, o expf(power)), test_T = T (1 - alpha), C = fma(T, alpha c, C) -- so pixels,
 // final_T and n_contrib are bit-identical.  A pair that does not blend is carried as alpha = 0, which leaves C and T
@@ -311,14 +310,14 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
                         mm &= mm - 1;
                         const FwdPairRec& R = s_rec[buf][j];
                         const float4 xy = R.xy, ac = R.ac, bo = R.bo;
-                        const float2 dx = __fadd2_rn(make_float2(xy.x, xy.y), npx), dy = __fadd2_rn(make_float2(xy.z, xy.w), npy);
-                        const float2 t1 = __fmul2_rn(make_float2(ac.x, ac.y), dx);
-                        const float2 t3 = __fmul2_rn(dy, __fmul2_rn(make_float2(ac.z, ac.w), dy));
-                        const float2 un = __fmul2_rn(dy, __fmul2_rn(make_float2(bo.x, bo.y), dx));     // -(B dx) dy
-                        const float2 power = __ffma2_rn(__ffma2_rn(dx, t1, t3), mhalf, un);
-                        const float2 oG = __fmul2_rn(make_float2(bo.z, bo.w), make_float2(expf(power.x), expf(power.y)));
+                        const float2 dx = add2(make_float2(xy.x, xy.y), npx), dy = add2(make_float2(xy.z, xy.w), npy);
+                        const float2 t1 = mul2(make_float2(ac.x, ac.y), dx);
+                        const float2 t3 = mul2(dy, mul2(make_float2(ac.z, ac.w), dy));
+                        const float2 un = mul2(dy, mul2(make_float2(bo.x, bo.y), dx));     // -(B dx) dy
+                        const float2 power = fma2(fma2(dx, t1, t3), mhalf, un);
+                        const float2 oG = mul2(make_float2(bo.z, bo.w), make_float2(expf(power.x), expf(power.y)));
                         const float a0 = min(0.99f, oG.x), a1 = min(0.99f, oG.y);
-                        const float2 test_T = __fmul2_rn(T, __fadd2_rn(one, make_float2(-a0, -a1)));
+                        const float2 test_T = mul2(T, add2(one, make_float2(-a0, -a1)));
                         const bool blend0 = live0 && !(power.x > 0.0f) && !(a0 < 1.0f / 255.0f);
                         const bool blend1 = live1 && !(power.y > 0.0f) && !(a1 < 1.0f / 255.0f);
                         const bool stop0 = blend0 && test_T.x < 0.0001f, stop1 = blend1 && test_T.y < 0.0001f;
@@ -328,9 +327,9 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
                         if (!__any_sync(0xFFFFFFFFu, upd0 || upd1)) continue;
                         const float2 alpha = make_float2(upd0 ? a0 : 0.f, upd1 ? a1 : 0.f);
                         const float4 rg = R.rg, bb = R.bb;
-                        C0 = __ffma2_rn(T, __fmul2_rn(alpha, make_float2(rg.x, rg.y)), C0);
-                        C1 = __ffma2_rn(T, __fmul2_rn(alpha, make_float2(rg.z, rg.w)), C1);
-                        C2 = __ffma2_rn(T, __fmul2_rn(alpha, make_float2(bb.x, bb.y)), C2);
+                        C0 = fma2(T, mul2(alpha, make_float2(rg.x, rg.y)), C0);
+                        C1 = fma2(T, mul2(alpha, make_float2(rg.z, rg.w)), C1);
+                        C2 = fma2(T, mul2(alpha, make_float2(bb.x, bb.y)), C2);
                         T = make_float2(upd0 ? test_T.x : T.x, upd1 ? test_T.y : T.y);
                         // 1-based position of this instance in the tile's list (forward.cu:349,382)
                         const uint32_t idx = round_base + (uint32_t)j + 1u;

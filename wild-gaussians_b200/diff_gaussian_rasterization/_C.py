@@ -290,7 +290,7 @@ def rasterize_gaussians_shard(shard, background, means3D, colors, opacity, scale
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     if not means3D.is_cuda:
-        raise RuntimeError("diff_gaussian_rasterization (sm_100a build) needs CUDA tensors; there is no CPU path")
+        raise RuntimeError("diff_gaussian_rasterization (sm_90a build) needs CUDA tensors; there is no CPU path")
     dev = means3D.device
     P, H, W = int(means3D.size(0)), int(image_height), int(image_width)
     shard = _abi_shard(shard, H)
@@ -581,7 +581,7 @@ def rasterize_gaussians_backward_finalize(accum, *args, shard=None):
 def mark_visible(means3D, viewmatrix, projmatrix):
     """Drop-in for ``markVisible`` (rasterize_points.cu:206-225): bool[P], view-space z > 0.2."""
     if not means3D.is_cuda:
-        raise RuntimeError("diff_gaussian_rasterization (sm_100a build) needs CUDA tensors; there is no CPU path")
+        raise RuntimeError("diff_gaussian_rasterization (sm_90a build) needs CUDA tensors; there is no CPU path")
     dev = means3D.device
     P = int(means3D.size(0))
     with torch.cuda.device(dev):

@@ -1,4 +1,4 @@
-"""Drop-in ``diff_gaussian_rasterization`` package backed by the sm_100a rasterizer.
+"""Drop-in ``diff_gaussian_rasterization`` package backed by the sm_90a rasterizer.
 
 Public surface = the reference's (``submodules/diff-gaussian-rasterization/
 diff_gaussian_rasterization/__init__.py``):

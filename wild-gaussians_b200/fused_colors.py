@@ -3,7 +3,7 @@
 ``fused_colors(...)`` returns the two colour sets ``GaussianModel._render_internal`` feeds the rasterizer -- the raw
 SH colours (method.py:1571-1579) and the appearance-toned colours (method.py:1586-1598, ``EmbeddingModel.forward``
 :889-900, ``eval_sh`` :493-548) -- from the model's raw parameters, with full autograd support, in ONE kernel per
-direction: the 59 -> 128 -> 128 -> 6 MLP runs on tcgen05 tensor cores (bf16 operands, fp32 accumulation in TMEM),
+direction: the 59 -> 128 -> 128 -> 6 MLP runs on wgmma tensor cores (bf16 operands, fp32 accumulation),
 the activations never leave the SM.  Opt-in: ``wildgaussians/method.py`` itself is untouched;
 ``wildgaussians_fused.enable(model)`` swaps the caller.
 

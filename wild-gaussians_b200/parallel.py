@@ -98,9 +98,9 @@ def reduce_partials(accum: torch.Tensor, group=None) -> torch.Tensor:
 # GSR_PEER_REDUCE=3 ("pull"): the backward composite adds into its OWN accumulator and marks the Gaussians it touched; after
 # one barrier every rank's chain-rule kernel reads the marked rows of the other ranks through their peer mappings (plain
 # loads, rank order -> bit-identical gradients on all ranks).  No remote atomics: peer `red` is posted cheaply but drains
-# slowly (measured at 4 GPUs: 0.37 ms of the 1.21-ms step are hidden behind the barrier that follows the kernel).
-# Default (GSR_PEER_REDUCE unset): 1 for two ranks, 3 from three ranks on -- measured on B200s at C3: 2 GPUs 1.12 ms (mode 1) vs
-# 1.19 (mode 3); 4 GPUs 1.21 (mode 1) vs 0.92 (mode 2) vs 0.91 (mode 3).
+# slowly, behind the barrier that follows the kernel.
+# Default (GSR_PEER_REDUCE unset): 1 for two ranks, 3 from three ranks on (the remote-atomic drain grows with the rank
+# count; the multi-GPU modes have not been timed on H100 machines).
 _PEER_MODE_ENV = os.environ.get("GSR_PEER_REDUCE")
 
 

@@ -8,7 +8,7 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 
 * evaluates the parameter activations + 3D filter (``get_gaussians``, method.py:1060-1086) with one kernel per direction;
 * evaluates the raw and the appearance-toned colours with ONE fused kernel per direction (``fused_colors``:
-  tcgen05 MLP + SH evaluation, ``csrc/appearance.cu``) instead of ~60 PyTorch launches and several P x 128 / P x 48
+  wgmma MLP + SH evaluation, ``csrc/appearance.cu``) instead of ~60 PyTorch launches and several P x 128 / P x 48
   fp32 intermediates (method.py:1570-1598);
 * caches the per-camera constants -- the numpy 4x4 inversions, ``getWorld2View2``, the projection matrix, the camera
   centre, tan(fov) (method.py:1502-1527) -- per (pose, intrinsics, size), and the all-zero ``subpixel_offset`` /
