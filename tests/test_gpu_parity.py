@@ -83,7 +83,7 @@ REF_SCENES = [
     dict(P=60_000, W=400, H=300, sh_degree=None, seed=26, cov3D_precomp=True),
     # more than 256 binning cells (8x8 tiles each): the coarse-item sort needs two radix passes
     dict(P=150_000, W=4096, H=2304, sh_degree=None, seed=27),
-    # medium-to-large splats: binning units whose output exceeds the staging buffer (two-walk / direct scatter paths)
+    # medium-to-large splats: binning units whose output exceeds the staging buffer (multi-walk scatter)
     dict(P=100_000, W=1280, H=720, sh_degree=None, seed=28, scale_range=(0.01, 0.15)),
     # SH tensors with 4 coefficients (128-bit row accesses) and 9 coefficients (rows not 16-byte multiples: scalar path)
     dict(P=30_000, W=320, H=240, sh_degree=1, max_sh_degree=1, seed=29),

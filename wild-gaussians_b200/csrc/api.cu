@@ -87,8 +87,7 @@ size_t carve_geom(char* base, int P, int M, GeomState* out) {
     take(cur, g.cells_sorted, n);
     take(cur, g.rect_sorted, n);
     take(cur, g.offsets, n + 1);
-    g.radix_tmp_count = radix_tmp_elems(n) + scan_tmp_elems(n);
-    take(cur, g.radix_tmp, g.radix_tmp_count);
+    take(cur, g.radix_tmp, radix_tmp_elems(n) + scan_tmp_elems(n));
     if (out) *out = g;
     return (size_t)(cur - base) + 256;
 }
@@ -129,9 +128,8 @@ size_t carve_bin_scratch(char* base, size_t N1, int W, int H, BinScratch* out) {
     b.units_cap = ((N1 / UNIT + num_cells + 7) / 8) * 8;
     take(cur, b.M, (size_t)CELL_TILES * b.units_cap);
     take(cur, b.row_total, CELL_TILES);
-    take(cur, b.tile_count, num_tiles + 1);
     take(cur, b.tile_start, num_tiles + 1);
-    take(cur, b.scan_tmp, scan_tmp_elems(num_tiles));
+    take(cur, b.block_sums, (num_tiles + 1023) / 1024);
     if (out) *out = b;
     return (size_t)(cur - base) + 256;
 }
@@ -241,10 +239,10 @@ static int geometry_stage(const GsrForwardArgs* a, const GeomState& g, int ty0, 
 
     // coarse-item offsets in depth order; the total (number of coarse items) goes to counters[4]
     prof_begin(ST_OFFSET_SCAN, s);
-    rc = scan_gathered(g.cells_sorted, nullptr, g.offsets, (size_t)a->P, g.radix_tmp + radix_tmp_elems((size_t)a->P), s, n_sorted,
-                       reinterpret_cast<uint32_t*>(g.counters + 4));
+    rc = exclusive_scan_u32(g.cells_sorted, g.offsets, (size_t)a->P, g.radix_tmp + radix_tmp_elems((size_t)a->P), s,
+                            n_sorted, reinterpret_cast<uint32_t*>(g.counters + 4));
     if (rc) return rc;
-    GSR_STAGE(s, dbg, "scan_gathered");
+    GSR_STAGE(s, dbg, "exclusive_scan_u32");
     prof_end(ST_OFFSET_SCAN, s);
     return 0;
 }

@@ -24,7 +24,6 @@
 // N4).  Traffic is about 4 bytes per instance (the list itself) plus a few tens of bytes per Gaussian.
 // No spin-waits anywhere: every kernel is a plain data-parallel launch.
 #include "common.cuh"
-#include <cstdlib>
 
 namespace gsr {
 
@@ -91,21 +90,11 @@ __global__ void __launch_bounds__(256) cell_bounds_kernel(const uint32_t* __rest
 __device__ __forceinline__ void block_scan2_1024(uint32_t& a, uint32_t& b, uint32_t* s_warp_a, uint32_t* s_warp_b,
                                                  uint32_t* s_carry, uint32_t& excl_a, uint32_t& excl_b) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t xa = a, xb = b;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t ya = __shfl_up_sync(0xFFFFFFFFu, xa, o), yb = __shfl_up_sync(0xFFFFFFFFu, xb, o);
-        if (lane >= o) { xa += ya; xb += yb; }
-    }
+    const uint32_t xa = warp_inclusive_scan(a), xb = warp_inclusive_scan(b);
     if (lane == 31) { s_warp_a[warp] = xa; s_warp_b[warp] = xb; }
     __syncthreads();
     if (warp == 0) {
-        uint32_t wa = s_warp_a[lane], wb = s_warp_b[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t ya = __shfl_up_sync(0xFFFFFFFFu, wa, o), yb = __shfl_up_sync(0xFFFFFFFFu, wb, o);
-            if (lane >= o) { wa += ya; wb += yb; }
-        }
+        const uint32_t wa = warp_inclusive_scan(s_warp_a[lane]), wb = warp_inclusive_scan(s_warp_b[lane]);
         s_warp_a[lane] = wa; s_warp_b[lane] = wb;
     }
     __syncthreads();
@@ -273,67 +262,18 @@ __global__ void __launch_bounds__(1024) tile_offsets_lookback_kernel(const uint3
 }
 
 // ---- level 2c: scatter ------------------------------------------------------------------------------
-// One warp per unit.  Lane l owns the running output position of local tiles l and l + 32 (column l & 7, rows
-// l >> 3 and 4 + (l >> 3) of the cell).  The unit's coarse items are walked IN ORDER, 32 at a time: every lane
-// first turns its own item into an 8-bit column mask and an 8-bit row mask (staged in shared memory with the
-// Gaussian id), then the warp loops over the staged items and each lane appends the id to the lists of the tiles
-// it owns -- no ballots, no ranks: the order inside a tile list is the walk order = depth order.
-__global__ void __launch_bounds__(256) cell_scatter_kernel(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                                                           const uint32_t* __restrict__ unit_base,
-                                                           const uint2* __restrict__ cell_range, uint32_t num_cells,
-                                                           const uint32_t* __restrict__ Pm, const uint32_t* __restrict__ row_total,
-                                                           uint32_t cap, const uint32_t* __restrict__ tile_start, int cells_x,
-                                                           int grid_x, int grid_y, uint32_t* __restrict__ point_list) {
-    __shared__ uint2 s_item[8][32];   // {column mask | row mask << 8, Gaussian id}
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t u = blockIdx.x * 8 + warp;
-    const uint32_t num_units = unit_base[num_cells];
-    if (u >= num_units) return;
-    const UnitInfo ui = unit_info(unit_base, cell_range, num_cells, u);
-    uint32_t pos[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const uint32_t t = lane + 32 * h;
-        const int tx = (int)(ui.cell % cells_x) * CELL + (int)(t % CELL), ty = (int)(ui.cell / cells_x) * CELL + (int)(t / CELL);
-        uint32_t p = 0;
-        if (tx < grid_x && ty < grid_y)
-            p = tile_start[ty * grid_x + tx] + prefix_at(Pm, row_total, cap, t, u) -
-                prefix_at(Pm, row_total, cap, t, ui.first_unit_of_cell);
-        pos[h] = p;
-    }
-    const int sx = lane & 7, sy0 = 8 + (lane >> 3), sy1 = 12 + (lane >> 3);
-    for (uint32_t base = 0; base < ui.count; base += 32) {
-        const int nitems = (int)min(32u, ui.count - base);
-        __syncwarp();
-        if (lane < nitems) {
-            const uint32_t key = keys[ui.first + base + lane];
-            const uint32_t x0 = (key >> 16) & 15u, y0 = (key >> 20) & 15u, x1 = (key >> 24) & 15u, y1 = (key >> 28) & 15u;
-            const uint32_t cm = ((1u << x1) - 1u) & ~((1u << x0) - 1u);
-            const uint32_t rm = ((1u << y1) - 1u) & ~((1u << y0) - 1u);
-            s_item[warp][lane] = make_uint2(cm | (rm << 8), vals[ui.first + base + lane]);
-        }
-        __syncwarp();
-#pragma unroll 4
-        for (int i = 0; i < nitems; ++i) {
-            const uint2 it = s_item[warp][i];
-            const uint32_t c = it.x >> sx;
-            if (c & (it.x >> sy0) & 1u) point_list[pos[0]++] = it.y;
-            if (c & (it.x >> sy1) & 1u) point_list[pos[1]++] = it.y;
-        }
-    }
-}
-
-// ---- level 2c': staged scatter ------------------------------------------------------------------------
-// Same walk as cell_scatter_kernel, but a unit's output is first assembled in shared memory, tile run after
-// tile run, and then copied to the tile lists with coalesced stores.  The run lengths of the unit are known
-// exactly -- they are the differences of the row-scanned count matrix -- so every tile gets a fixed slice of the
-// staging buffer (exclusive scan over the cell's 64 tiles) and an append is one predicated STS through a lane-private
-// pointer.  Per coarse item the warp reads one 16-byte record {coverage bits of tiles 0-31, of tiles 32-63, id}
-// and each lane tests "its" bit of the two words.
-// The direct version issues one 4-byte global store per (lane, entry) into 64 different lists: at C3 (37.6 M
-// entries) ncu shows 37.5 M single-sector L2 write requests, 227 MB DRAM written + 159 MB read back for partial
-// sectors, 0.36 ms.  Staging turns them into ~3 M requests.
-// A unit whose output does not fit the staging buffer (very large splats) takes the direct path.
+// One warp per unit.  Lane l owns local tiles l and l + 32 of the cell.  The unit's coarse items are walked IN
+// ORDER, 32 at a time, and each lane appends the ids of the items covering its tiles -- no ballots, no ranks: the
+// order inside a tile list is the walk order = depth order.  The unit's output is first assembled in shared memory,
+// tile run after tile run, and then copied to the tile lists with coalesced stores.  The run lengths of the unit
+// are known exactly -- they are the differences of the row-scanned count matrix -- so every tile gets a fixed slice
+// of the staging buffer (exclusive scan over the cell's 64 tiles) and an append is one predicated STS through a
+// lane-private pointer.  Per coarse item the warp reads one 16-byte record {coverage bits of tiles 0-31, of tiles
+// 32-63, id} and each lane tests "its" bit of the two words.
+// Why staging: direct per-lane global stores (one 4-byte store per (lane, entry) into 64 different lists) gave 37.5 M
+// single-sector L2 write requests at C3 (37.6 M entries), 227 MB DRAM written + 159 MB read back for partial
+// sectors; staging turns them into ~3 M requests.
+// A unit whose output does not fit the staging buffer (very large splats) is staged in several walks.
 constexpr int SQ_ENTRIES = 2048;           // staging capacity per warp (a unit of 256 items averages ~1800 at C3)
 constexpr int SQ_WARPS = 8;
 constexpr int SQ_WARP_WORDS = SQ_ENTRIES + 32 * 4;           // staging + 32 item records (uint4)
@@ -434,12 +374,7 @@ __global__ void __launch_bounds__(SQ_WARPS * 32) cell_scatter_staged_kernel(
     // exclusive prefix of the run lengths in tile order (0..63): the staging slice of every tile
     uint32_t pre[2];
     {
-        uint32_t x0 = len[0], x1 = len[1];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y0 = __shfl_up_sync(0xFFFFFFFFu, x0, o), y1 = __shfl_up_sync(0xFFFFFFFFu, x1, o);
-            if (lane >= o) { x0 += y0; x1 += y1; }
-        }
+        const uint32_t x0 = warp_inclusive_scan(len[0]), x1 = warp_inclusive_scan(len[1]);
         const uint32_t tot0 = __shfl_sync(0xFFFFFFFFu, x0, 31);
         pre[0] = x0 - len[0];
         pre[1] = tot0 + x1 - len[1];
@@ -526,7 +461,7 @@ int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R_cap, size
     const uint32_t cap = (uint32_t)bs.units_cap;
     if (radix_num_passes(0, cell_bits) == 1) {
         // one pass sorted by the whole cell id: its digit totals ARE the items per cell
-        build_units_kernel<<<1, 1024, 0, s>>>(bs.cell_range, num_cells, bs.unit_base, radix_pass_totals(bs.radix_tmp, N1, 1));
+        build_units_kernel<<<1, 1024, 0, s>>>(bs.cell_range, num_cells, bs.unit_base, radix_pass_totals(bs.radix_tmp, N1));
         count_launches(1);
     } else {
         GSR_CUDA(cudaMemsetAsync(bs.cell_range, 0, (size_t)num_cells * sizeof(uint2), s));
@@ -547,10 +482,9 @@ int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R_cap, size
     if (rc) return rc;
     const int off_ctas = (num_tiles + 1023) / 1024;
     if (off_ctas > 1 && off_ctas <= 120) {
-        unsigned long long* block_sums = reinterpret_cast<unsigned long long*>(bs.tile_count);     // [T+1] words, 256-B aligned, otherwise unused
-        GSR_CUDA(cudaMemsetAsync(block_sums, 0, (size_t)off_ctas * sizeof(unsigned long long), s));
+        GSR_CUDA(cudaMemsetAsync(bs.block_sums, 0, (size_t)off_ctas * sizeof(unsigned long long), s));
         tile_offsets_lookback_kernel<<<off_ctas, 1024, 0, s>>>(bs.M, bs.row_total, bs.unit_base, cap, cells_x, gx, num_tiles,
-                                                               bs.tile_start, ranges, block_sums);
+                                                               bs.tile_start, ranges, bs.block_sums);
     } else {
         tile_offsets_kernel<<<1, 1024, 0, s>>>(bs.M, bs.row_total, bs.unit_base, cap, cells_x, gx, num_tiles, bs.tile_start, ranges);
     }
@@ -559,24 +493,14 @@ int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R_cap, size
     prof_end(ST_TILE_OFFSETS, s);
     prof_begin(ST_TILE_SCATTER, s);
 
-    static int impl = -1;
-    if (impl < 0) {
-        const char* e = getenv("GSR_SCATTER");       // tuning aid: 0 = direct per-lane stores, 1 = shared-memory staged
-        impl = e ? atoi(e) : 1;
-    }
     // function attributes are per device / context: set it for the current device on every call (a process may
     // rasterize on several GPUs), it is a cheap driver call
-    if (impl != 0)
-        GSR_CUDA(cudaFuncSetAttribute(cell_scatter_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SQ_SMEM));
-    if (impl == 0)
-        cell_scatter_kernel<<<(cap + 7) / 8, 256, 0, s>>>(keys, vals, bs.unit_base, bs.cell_range, num_cells, bs.M, bs.row_total,
-                                                          cap, bs.tile_start, cells_x, gx, gy, point_list);
-    else
-        cell_scatter_staged_kernel<<<(cap + SQ_WARPS - 1) / SQ_WARPS, SQ_WARPS * 32, SQ_SMEM, s>>>(
-            keys, vals, bs.unit_base, bs.cell_range, num_cells, bs.M, bs.row_total, cap, bs.tile_start, cells_x, gx, gy,
-            point_list);
+    GSR_CUDA(cudaFuncSetAttribute(cell_scatter_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SQ_SMEM));
+    cell_scatter_staged_kernel<<<(cap + SQ_WARPS - 1) / SQ_WARPS, SQ_WARPS * 32, SQ_SMEM, s>>>(
+        keys, vals, bs.unit_base, bs.cell_range, num_cells, bs.M, bs.row_total, cap, bs.tile_start, cells_x, gx, gy,
+        point_list);
     count_launches(1);
-    GSR_STAGE(s, debug, "cell_scatter_kernel");
+    GSR_STAGE(s, debug, "cell_scatter_staged_kernel");
     prof_end(ST_TILE_SCATTER, s);
     return 0;
 }

@@ -67,7 +67,6 @@ struct GeomState {
     TileRect* rect_sorted;    // [P]  tile rectangles in depth order (written by the last sort pass)
     uint32_t* offsets;        // [P+1] exclusive scan of cells_touched in depth order
     uint32_t* radix_tmp;      // histogram / scan temporaries
-    size_t    radix_tmp_count;
 };
 
 struct ImgState {
@@ -91,9 +90,8 @@ struct BinScratch {           // transient state of the two-level tile binning (
     size_t    units_cap;      // upper bound of the number of units: N1 / UNIT + NC, rounded up to 8
     uint32_t* M;              // [64][units_cap] per-(local tile, unit) counts, then their row-wise prefix
     uint32_t* row_total;      // [64]
-    uint32_t* tile_count;     // [T+1]
     uint32_t* tile_start;     // [T+1]
-    uint32_t* scan_tmp;
+    unsigned long long* block_sums;   // [ceil(T / 1024)] per-CTA tile totals of tile_offsets_lookback_kernel
 };
 
 size_t carve_geom(char* base, int P, int M, GeomState* out);       // returns bytes used
@@ -127,14 +125,26 @@ int radix_sort_pairs(uint32_t* key_a, uint32_t* val_a, uint32_t* key_b, uint32_t
                      int begin_bit, int end_bit, uint32_t* tmp, cudaStream_t s, bool debug, const RadixAux* aux = nullptr,
                      const uint32_t* n_dev = nullptr, uint32_t* n_compact = nullptr);
 // digit totals (RADIX entries) left in `tmp` by the most recent pass of radix_sort_pairs over n items
-const uint32_t* radix_pass_totals(const uint32_t* tmp, size_t n, int passes);
-// exclusive scan of gathered counts: out[i] = sum_{j<i} counts[perm[j]], out[n] = total
-int scan_gathered(const uint32_t* counts, const uint32_t* perm, uint32_t* out, size_t n_cap,
-                  uint32_t* tmp, cudaStream_t s, const uint32_t* n_dev = nullptr, uint32_t* total_out = nullptr);
+const uint32_t* radix_pass_totals(const uint32_t* tmp, size_t n);
+// exclusive scan of counts: out[i] = sum_{j<i} counts[j], out[n] = total
+int exclusive_scan_u32(const uint32_t* counts, uint32_t* out, size_t n_cap, uint32_t* tmp, cudaStream_t s,
+                       const uint32_t* n_dev = nullptr, uint32_t* total_out = nullptr);
 size_t scan_tmp_elems(size_t n);
 
 // in-place exclusive scan along each row of a [rows][cols] u32 matrix; row sums -> total[rows]
 int row_scan_u32(uint32_t* m, int rows, size_t cols, uint32_t* total, cudaStream_t s);
+
+// inclusive prefix sum over the 32 lanes of a warp; every lane of the warp must call it
+__device__ __forceinline__ uint32_t warp_inclusive_scan(uint32_t x) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+        if (lane >= o) x += y;
+    }
+    return x;
+}
+
 // per-tile instance lists + ranges from the depth-ordered Gaussians (binning.cu)
 int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R, size_t N1, const BinScratch& bs,
                      uint32_t* point_list, uint2* ranges, cudaStream_t s, bool debug);

@@ -405,17 +405,10 @@ int launch_preprocess_bwd(const GsrBackwardArgs& a, const GeomState& g, BwdAccum
     p.dL_dmean2D = a.dL_dmean2D; p.dL_dconic = a.dL_dconic; p.dL_dopacity = a.dL_dopacity;
     p.dL_dcolor = a.dL_dcolor; p.dL_dmean3D = a.dL_dmean3D; p.dL_dcov3D = a.dL_dcov3D;
     p.dL_dsh = a.dL_dsh; p.dL_dscale = a.dL_dscale; p.dL_drot = a.dL_drot;
-    static int occ = -1;
-    if (occ < 0) {
-        const char* e = getenv("GSR_PREBWD_OCC");    // tuning aid: resident CTAs per SM the register allocation targets
-        occ = e ? atoi(e) : 4;
-    }
     p.sh_vec = a.shs != nullptr && (a.M == 4 || a.M == 16) &&
                (reinterpret_cast<uintptr_t>(a.shs) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a.dL_dsh) & 15u) == 0;
     if (a.shs != nullptr) preprocess_bwd_kernel<2, true><<<(a.P + 255) / 256, 256, 0, s>>>(p);   // 48 + 16 extra live registers
-    else if (occ >= 4) preprocess_bwd_kernel<4, false><<<(a.P + 255) / 256, 256, 0, s>>>(p);
-    else if (occ == 3) preprocess_bwd_kernel<3, false><<<(a.P + 255) / 256, 256, 0, s>>>(p);
-    else preprocess_bwd_kernel<2, false><<<(a.P + 255) / 256, 256, 0, s>>>(p);
+    else preprocess_bwd_kernel<4, false><<<(a.P + 255) / 256, 256, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

@@ -1,5 +1,5 @@
 // radix.cu -- stable LSD radix partition of (u32 key, u32 value) pairs and an exclusive scan
-// of gathered counts.  Hand-written replacement for the two CUB calls on the reference's
+// of counts.  Hand-written replacement for the two CUB calls on the reference's
 // path (cub::DeviceRadixSort::SortPairs, rasterizer_impl.cu:303-311, and
 // cub::DeviceScan::InclusiveSum, :280).
 //
@@ -11,7 +11,7 @@
 //
 // One pass = three launches, no spin-waiting between CTAs (so nothing can dead-lock):
 //   radix_hist_kernel    per-CTA digit histogram of a CHUNK of the input (plain shared atomics) -> hist[digit][cta]
-//   radix_rowscan_kernel one CTA per digit: exclusive scan along the row    -> hist (in place), total[digit]
+//   rowscan_wide_kernel  one CTA per digit: exclusive scan along the row    -> hist (in place), total[digit]
 //   radix_scatter_kernel re-reads the chunk, ranks every item among equal digits in (warp, round, lane) = input
 //                        order -- the lanes holding the same digit are found with 8 ballots, one per digit bit;
 //                        __match_any_sync was measured 2-4x slower here because its cost grows with the number of
@@ -19,7 +19,6 @@
 //                        that consecutive threads write consecutive addresses inside every digit run.
 // The last pass of a sort can also deliver side data in sorted order (RadixAux).
 #include "common.cuh"
-#include <cstdlib>
 
 namespace gsr {
 
@@ -33,12 +32,8 @@ constexpr int RS_WARP_ITEMS = 32 * RS_ITEMS;       // items per warp (contiguous
 
 static inline size_t radix_ctas(size_t n) { return (n + RS_CHUNK - 1) / RS_CHUNK; }
 
-constexpr int OS_MAX_PASSES = 4;
-size_t radix_tmp_elems(size_t n) {
-    // three-kernel path: hist[RADIX][ctas] + total[RADIX]
-    // one-launch path:   ghist[4][RADIX] + tickets / error flag [64] + status[4][ctas][RADIX]
-    return (size_t)RADIX * (OS_MAX_PASSES * radix_ctas(n) + OS_MAX_PASSES + 1) + 128;
-}
+// hist[RADIX][ctas] + total[RADIX]
+size_t radix_tmp_elems(size_t n) { return (size_t)RADIX * (radix_ctas(n) + 1); }
 
 // The item count is min(*n_dev, n_cap) when n_dev != NULL (the grid is sized for n_cap; CTAs beyond the count publish
 // zero histogram columns).  DROP: keys equal to RADIX_DROP_KEY are not part of the sort at all (neither counted nor
@@ -82,49 +77,10 @@ __global__ void __launch_bounds__(RS_THREADS) radix_hist_kernel(const uint32_t* 
     for (int i = threadIdx.x; i < RADIX; i += RS_THREADS) hist[(size_t)i * ctas + blockIdx.x] = s_hist[i];
 }
 
-// one CTA per digit; exclusive scan of hist[digit][0..ctas) in place, row total -> total[digit]
-__global__ void __launch_bounds__(1024) radix_rowscan_kernel(uint32_t* __restrict__ hist, uint32_t ctas,
-                                                             uint32_t* __restrict__ total) {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    uint32_t* row = hist + (size_t)blockIdx.x * ctas;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < ctas; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const uint32_t v = i < ctas ? row[i] : 0u;
-        uint32_t x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t w = s_warp[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, w, o);
-                if (lane >= o) w += y;
-            }
-            s_warp[lane] = w;  // inclusive over warps
-        }
-        __syncthreads();
-        const uint32_t warp_excl = warp == 0 ? 0u : s_warp[warp - 1];
-        const uint32_t carry = s_carry;
-        if (i < ctas) row[i] = carry + warp_excl + x - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = carry + s_warp[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) total[blockIdx.x] = s_carry;
-}
-
-// The same scan for LONG rows (the count matrix of the tile binning: 64 rows of ~20 k columns): K chunks of 1024 columns per
-// round share the two barriers of a round (warp w combines the warp totals of chunk w), so a row costs cols / (K * 1024)
-// dependent rounds instead of cols / 1024; loads and stores stay coalesced.
+// One CTA per row of a [rows][cols] matrix: exclusive scan of the row in place, row total -> total[row].  K chunks of 1024
+// columns per round share the two barriers of a round (warp w combines the warp totals of chunk w), so a LONG row (the
+// count matrix of the tile binning: 64 rows of ~20 k columns) costs cols / (K * 1024) dependent rounds instead of
+// cols / 1024; loads and stores stay coalesced.  K = 1 for short rows (radix histograms, scan partials).
 template <int K>
 __global__ void __launch_bounds__(1024) rowscan_wide_kernel(uint32_t* __restrict__ hist, uint32_t cols, uint32_t* __restrict__ total) {
     __shared__ uint32_t s_warp[K][32];
@@ -142,24 +98,11 @@ __global__ void __launch_bounds__(1024) rowscan_wide_kernel(uint32_t* __restrict
         }
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            x[k] = v[k];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x[k], o);
-                if (lane >= o) x[k] += y;
-            }
+            x[k] = warp_inclusive_scan(v[k]);
             if (lane == 31) s_warp[k][warp] = x[k];
         }
         __syncthreads();
-        if (warp < K) {
-            uint32_t w = s_warp[warp][lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, w, o);
-                if (lane >= o) w += y;
-            }
-            s_warp[warp][lane] = w;      // inclusive over the warps of chunk `warp`
-        }
+        if (warp < K) s_warp[warp][lane] = warp_inclusive_scan(s_warp[warp][lane]);   // inclusive over the warps of chunk `warp`
         __syncthreads();
         uint32_t off = s_carry;
 #pragma unroll
@@ -210,12 +153,7 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint32_
     {
         __shared__ uint32_t s_w[RS_WARPS];
         const uint32_t v = total[threadIdx.x];
-        uint32_t x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-            if (lane >= o) x += y;
-        }
+        const uint32_t x = warp_inclusive_scan(v);
         if (lane == 31) s_w[warp] = x;
         __syncthreads();
         uint32_t off = 0;
@@ -267,12 +205,7 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint32_
         uint32_t c[RS_WARPS];
 #pragma unroll
         for (int w = 0; w < RS_WARPS; ++w) { c[w] = s_cnt[w][d]; run += c[w]; }
-        uint32_t x = run;     // inclusive scan of the digit totals of this CTA
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-            if (lane >= o) x += y;
-        }
+        const uint32_t x = warp_inclusive_scan(run);     // inclusive scan of the digit totals of this CTA
         if (lane == 31) s_w2[warp] = x;
         __syncthreads();
         uint32_t off = 0;
@@ -314,234 +247,13 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint32_
     }
 }
 
-// ---- one launch per pass: chained-scan with decoupled look-back ------------------------------------------------------------
-// The three-kernel pass above reads the keys twice and needs two extra dependent launches (histogram, row scan) before its
-// scatter.  Here ONE upfront kernel histograms the digits of ALL passes (the multiset of keys does not change between
-// passes), and each pass is a single kernel: a CTA takes a ticket (its chunk index -- tickets are handed out in start
-// order, so every chunk a CTA waits for belongs to a CTA that is already running or finished: no dead-lock), ranks its
-// chunk, publishes its per-digit counts in a status word (2 flag bits + 30 count bits, one atomic word per (chunk, digit))
-// and looks back over the preceding chunks until it meets an inclusive prefix.  Waits are bounded: a lost status word
-// raises an error flag instead of hanging the GPU.
-constexpr uint32_t OS_AGG = 1u << 30, OS_PREFIX = 2u << 30, OS_COUNT = (1u << 30) - 1u;
-
-struct OnesweepTmp {
-    uint32_t* ghist;     // [OS_MAX_PASSES][RADIX] digit totals of every pass
-    uint32_t* ticket;    // [OS_MAX_PASSES] chunk tickets, [8] error flag
-    uint32_t* status;    // [OS_MAX_PASSES][ctas][RADIX]
-};
-static OnesweepTmp onesweep_tmp(uint32_t* tmp, uint32_t ctas) {
-    OnesweepTmp t;
-    t.ghist = tmp;
-    t.ticket = tmp + OS_MAX_PASSES * RADIX;
-    t.status = tmp + OS_MAX_PASSES * RADIX + 64;
-    (void)ctas;
-    return t;
-}
-
-template <bool DROP>
-__global__ void __launch_bounds__(RS_THREADS) radix_hist_all_kernel(const uint32_t* __restrict__ keys, size_t n_cap,
-                                                                    const uint32_t* __restrict__ n_dev, int begin_bit, int end_bit,
-                                                                    int passes, uint32_t* __restrict__ ghist) {
-    __shared__ uint32_t s_hist[OS_MAX_PASSES][RADIX];
-    const size_t n = radix_count(n_cap, n_dev);
-    const size_t base = (size_t)blockIdx.x * RS_CHUNK;
-    if (base >= n) return;
-    for (int i = threadIdx.x; i < OS_MAX_PASSES * RADIX; i += RS_THREADS) (&s_hist[0][0])[i] = 0;
-    __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const size_t i = base + (size_t)warp * RS_WARP_ITEMS + r * 32 + lane;
-        if (i < n) {
-            const uint32_t k = keys[i];
-            if (!(DROP && k == RADIX_DROP_KEY)) {
-                for (int p = 0; p < passes; ++p) {
-                    const int shift = begin_bit + p * RADIX_BITS;
-                    const uint32_t mask = (1u << min(RADIX_BITS, end_bit - shift)) - 1u;
-                    atomicAdd(&s_hist[p][(k >> shift) & mask], 1u);
-                }
-            }
-        }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < passes * RADIX; i += RS_THREADS) {
-        const uint32_t c = (&s_hist[0][0])[i];
-        if (c) atomicAdd(&ghist[i], c);
-    }
-}
-
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
-    asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-
-template <bool DROP, bool AUX>
-__global__ void __launch_bounds__(RS_THREADS) radix_onesweep_kernel(const uint32_t* __restrict__ keys_in,
-                                                                    const uint32_t* __restrict__ vals_in,
-                                                                    uint32_t* __restrict__ keys_out,
-                                                                    uint32_t* __restrict__ vals_out, size_t n_cap,
-                                                                    const uint32_t* __restrict__ n_dev, int shift, uint32_t mask,
-                                                                    const uint32_t* __restrict__ total,      // ghist of this pass
-                                                                    uint32_t* __restrict__ status, uint32_t* __restrict__ ticket,
-                                                                    uint32_t* __restrict__ error_flag, const RadixAux aux,
-                                                                    uint32_t* __restrict__ n_out) {
-    __shared__ uint32_t s_cnt[RS_WARPS][RADIX];   // per-warp digit counters, later chunk positions
-    __shared__ uint32_t s_digit_base[RADIX];
-    __shared__ uint32_t s_key[RS_CHUNK];
-    __shared__ uint32_t s_val[RS_CHUNK];
-    __shared__ uint32_t s_kept, s_chunk;
-    __shared__ uint32_t s_w[RS_WARPS], s_w2[RS_WARPS];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const size_t n = radix_count(n_cap, n_dev);
-    if (threadIdx.x == 0) s_chunk = atomicAdd(ticket, 1u);
-    for (int i = threadIdx.x; i < RS_WARPS * RADIX; i += RS_THREADS) (&s_cnt[0][0])[i] = 0;
-    __syncthreads();
-    const uint32_t chunk = s_chunk;
-
-    // exclusive scan of the digit totals (256 values, one per thread); chunk 0 also publishes the number of items
-    const uint32_t tot_d = total[threadIdx.x];
-    uint32_t tx = tot_d;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, tx, o);
-        if (lane >= o) tx += y;
-    }
-    if (lane == 31) s_w[warp] = tx;
-    __syncthreads();
-    uint32_t toff = 0, tall = 0;
-#pragma unroll
-    for (int w = 0; w < RS_WARPS; ++w) { if (w < warp) toff += s_w[w]; tall += s_w[w]; }
-    const uint32_t digit_global_base = toff + tx - tot_d;
-    if (n_out != nullptr && chunk == 0 && threadIdx.x == 0) *n_out = tall;
-    if ((size_t)chunk * RS_CHUNK >= n) return;
-
-    const size_t base = (size_t)chunk * RS_CHUNK + (size_t)warp * RS_WARP_ITEMS;
-    uint32_t key[RS_ITEMS], val[RS_ITEMS];
-    uint16_t rank[RS_ITEMS];
-    const unsigned lt_mask = (1u << lane) - 1u;
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const size_t i = base + r * 32 + lane;
-        const bool valid = i < n;
-        key[r] = valid ? keys_in[i] : RADIX_DROP_KEY;
-        val[r] = valid ? vals_in[i] : 0u;
-    }
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const size_t i = base + r * 32 + lane;
-        const bool valid = i < n && !(DROP && key[r] == RADIX_DROP_KEY);
-        const uint32_t d = valid ? ((key[r] >> shift) & mask) : 0u;
-        unsigned peers = __ballot_sync(0xFFFFFFFFu, valid);
-#pragma unroll
-        for (int b = 0; b < RADIX_BITS; ++b) {
-            const bool bit = (d >> b) & 1u;
-            const unsigned m = __ballot_sync(0xFFFFFFFFu, bit);
-            peers &= bit ? m : ~m;
-        }
-        uint32_t old = 0;
-        if (valid) old = s_cnt[warp][d];
-        __syncwarp();
-        if (valid && lane == (__ffs(peers) - 1)) s_cnt[warp][d] = old + __popc(peers);
-        __syncwarp();
-        rank[r] = (uint16_t)(old + __popc(peers & lt_mask));
-    }
-    __syncthreads();
-    {
-        // thread d: this chunk's count of digit d, its position inside the sorted chunk, and -- by look-back over the
-        // preceding chunks -- the number of items with digit d in front of this chunk
-        const int d = threadIdx.x;
-        uint32_t run = 0;
-        uint32_t c[RS_WARPS];
-#pragma unroll
-        for (int w = 0; w < RS_WARPS; ++w) { c[w] = s_cnt[w][d]; run += c[w]; }
-        uint32_t* my_status = status + (size_t)chunk * RADIX + d;
-        st_volatile_u32(my_status, (chunk == 0 ? OS_PREFIX : OS_AGG) | run);
-        uint32_t x = run;     // inclusive scan of the digit counts of this chunk
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_w2[warp] = x;
-        uint32_t before = 0;
-        if (chunk > 0) {
-            for (int64_t pc = (int64_t)chunk - 1; pc >= 0; --pc) {
-                const uint32_t* ps = status + (size_t)pc * RADIX + d;
-                uint32_t v = ld_volatile_u32(ps);
-                for (uint32_t spin = 0; (v >> 30) == 0u; ++spin) {
-                    if (spin > (1u << 24)) { atomicExch(error_flag, 1u); v = OS_PREFIX; break; }
-                    __nanosleep(20);
-                    v = ld_volatile_u32(ps);
-                }
-                before += v & OS_COUNT;
-                if ((v >> 30) == 2u) break;
-            }
-            st_volatile_u32(my_status, OS_PREFIX | ((before + run) & OS_COUNT));
-        }
-        __syncthreads();
-        uint32_t off = 0;
-        for (int w = 0; w < warp; ++w) off += s_w2[w];
-        uint32_t loc = off + x - run;   // first chunk position of digit d
-        if (d == RADIX - 1) s_kept = off + x;
-        s_digit_base[d] = digit_global_base + before - loc;   // global position = chunk position + s_digit_base[d]  (mod 2^32)
-#pragma unroll
-        for (int w = 0; w < RS_WARPS; ++w) { s_cnt[w][d] = loc; loc += c[w]; }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const size_t i = base + r * 32 + lane;
-        if (i < n && !(DROP && key[r] == RADIX_DROP_KEY)) {
-            const uint32_t d = (key[r] >> shift) & mask;
-            const uint32_t li = s_cnt[warp][d] + rank[r];
-            s_key[li] = key[r];
-            s_val[li] = val[r];
-        }
-    }
-    __syncthreads();
-    const uint32_t cta_n = s_kept;
-#pragma unroll 4
-    for (uint32_t i = threadIdx.x; i < cta_n; i += RS_THREADS) {
-        const uint32_t k = s_key[i];
-        const uint32_t pos = i + s_digit_base[(k >> shift) & mask];
-        keys_out[pos] = k;
-        const uint32_t v = s_val[i];
-        vals_out[pos] = v;
-        if (AUX) {
-            aux.out32[pos] = aux.in32[v];
-            aux.out64[pos] = aux.in64[v];
-        }
-    }
-}
-
-static int radix_impl() {
-    static int v = -1;
-    if (v < 0) {
-        // 0 (default) = three kernels per pass; 1 = one launch per pass.  Measured at C3: the one-launch passes are SLOWER
-        // (depth sort 0.244 vs 0.181 ms, cell sort 0.092 vs 0.049 ms): with 2048-item chunks a wave of ~900 CTAs starts
-        // together, every chunk's per-digit look-back walks serially over hundreds of "aggregate" status words
-        // (latency-bound, one dependent L2 read each) before it meets an inclusive prefix.  Kept for larger chunk sizes /
-        // a warp-parallel look-back (ROADMAP).
-        const char* e = getenv("GSR_RADIX");
-        v = e ? atoi(e) : 0;
-    }
-    return v;
-}
-
-// digit totals (RADIX entries) of the LAST pass of the most recent radix_sort_pairs over n_cap items with `passes` passes
-const uint32_t* radix_pass_totals(const uint32_t* tmp, size_t n, int passes) {
-    if (radix_impl() != 0 && passes <= OS_MAX_PASSES) return tmp + (size_t)(passes - 1) * RADIX;
-    return tmp + (size_t)RADIX * radix_ctas(n);
-}
+// digit totals (RADIX entries) of the LAST pass of the most recent radix_sort_pairs over n items
+const uint32_t* radix_pass_totals(const uint32_t* tmp, size_t n) { return tmp + (size_t)RADIX * radix_ctas(n); }
 
 int row_scan_u32(uint32_t* m, int rows, size_t cols, uint32_t* total, cudaStream_t s) {
     if (rows <= 0 || cols == 0) return 0;
     if (cols > 4096) rowscan_wide_kernel<8><<<rows, 1024, 0, s>>>(m, (uint32_t)cols, total);
-    else radix_rowscan_kernel<<<rows, 1024, 0, s>>>(m, (uint32_t)cols, total);
+    else rowscan_wide_kernel<1><<<rows, 1024, 0, s>>>(m, (uint32_t)cols, total);
     count_launches(1);
     GSR_CUDA(cudaGetLastError());
     return 0;
@@ -565,40 +277,6 @@ int radix_sort_pairs(uint32_t* key_a, uint32_t* val_a, uint32_t* key_b, uint32_t
     if (n_cap == 0) return 0;
     const int passes = radix_num_passes(begin_bit, end_bit);
     const uint32_t ctas = (uint32_t)radix_ctas(n_cap);
-    if (radix_impl() != 0 && passes <= OS_MAX_PASSES && n_cap < (size_t)OS_COUNT) {
-        const OnesweepTmp t = onesweep_tmp(tmp, ctas);
-        const size_t clear_words = (size_t)OS_MAX_PASSES * RADIX + 64 + (size_t)passes * ctas * RADIX;
-        GSR_CUDA(cudaMemsetAsync(tmp, 0, clear_words * sizeof(uint32_t), s));
-        if (n_compact) radix_hist_all_kernel<true><<<ctas, RS_THREADS, 0, s>>>(key_a, n_cap, n_dev, begin_bit, end_bit, passes, t.ghist);
-        else radix_hist_all_kernel<false><<<ctas, RS_THREADS, 0, s>>>(key_a, n_cap, n_dev, begin_bit, end_bit, passes, t.ghist);
-        count_launches(1);
-        GSR_STAGE(s, debug, "radix_hist_all_kernel");
-        for (int pass = 0; pass < passes; ++pass) {
-            const int shift = begin_bit + pass * RADIX_BITS;
-            const uint32_t mask = (1u << min(RADIX_BITS, end_bit - shift)) - 1u;
-            const bool a_to_b = (pass % 2) == 0;
-            const uint32_t* kin = a_to_b ? key_a : key_b;
-            const uint32_t* vin = a_to_b ? val_a : val_b;
-            uint32_t* kout = a_to_b ? key_b : key_a;
-            uint32_t* vout = a_to_b ? val_b : val_a;
-            const bool drop = n_compact != nullptr && pass == 0;
-            const uint32_t* nd = (n_compact != nullptr && pass > 0) ? n_compact : n_dev;
-            const bool with_aux = aux && pass == passes - 1;
-            const RadixAux ax = with_aux ? *aux : RadixAux{};
-            const uint32_t* tot = t.ghist + (size_t)pass * RADIX;
-            uint32_t* st = t.status + (size_t)pass * ctas * RADIX;
-            uint32_t* tk = t.ticket + pass;
-            uint32_t* ef = t.ticket + 8;
-            uint32_t* nout = drop ? n_compact : nullptr;
-            if (drop && with_aux) radix_onesweep_kernel<true, true><<<ctas, RS_THREADS, 0, s>>>(kin, vin, kout, vout, n_cap, nd, shift, mask, tot, st, tk, ef, ax, nout);
-            else if (drop) radix_onesweep_kernel<true, false><<<ctas, RS_THREADS, 0, s>>>(kin, vin, kout, vout, n_cap, nd, shift, mask, tot, st, tk, ef, ax, nout);
-            else if (with_aux) radix_onesweep_kernel<false, true><<<ctas, RS_THREADS, 0, s>>>(kin, vin, kout, vout, n_cap, nd, shift, mask, tot, st, tk, ef, ax, nout);
-            else radix_onesweep_kernel<false, false><<<ctas, RS_THREADS, 0, s>>>(kin, vin, kout, vout, n_cap, nd, shift, mask, tot, st, tk, ef, ax, nout);
-            count_launches(1);
-            GSR_STAGE(s, debug, "radix_onesweep_kernel");
-        }
-        return 0;
-    }
     uint32_t* hist = tmp;
     uint32_t* total = tmp + (size_t)RADIX * ctas;
     for (int pass = 0; pass < passes; ++pass) {
@@ -616,9 +294,9 @@ int radix_sort_pairs(uint32_t* key_a, uint32_t* val_a, uint32_t* key_b, uint32_t
         else radix_hist_kernel<false><<<ctas, RS_THREADS, 0, s>>>(kin, n_cap, nd, shift, mask, hist, ctas);
         count_launches(1);
         GSR_STAGE(s, debug, "radix_hist_kernel");
-        radix_rowscan_kernel<<<RADIX, 1024, 0, s>>>(hist, ctas, total);
+        rowscan_wide_kernel<1><<<RADIX, 1024, 0, s>>>(hist, ctas, total);
         count_launches(1);
-        GSR_STAGE(s, debug, "radix_rowscan_kernel");
+        GSR_STAGE(s, debug, "rowscan_wide_kernel");
         const bool with_aux = aux && pass == passes - 1;
         const RadixAux ax = with_aux ? *aux : RadixAux{};
         if (drop && with_aux) radix_scatter_kernel<true, true><<<ctas, RS_THREADS, 0, s>>>(kin, vin, kout, vout, n_cap, nd, shift, mask, hist, total, ctas, ax, n_compact);
@@ -632,7 +310,7 @@ int radix_sort_pairs(uint32_t* key_a, uint32_t* val_a, uint32_t* key_b, uint32_t
 }
 
 // ----------------------------------------------------------------------------------------
-// exclusive scan of counts gathered through a permutation (instance offsets in depth order)
+// exclusive scan of the depth-ordered cell counts (coarse-item offsets)
 // ----------------------------------------------------------------------------------------
 constexpr int SC_THREADS = 256;
 constexpr int SC_ITEMS = 8;
@@ -642,12 +320,7 @@ size_t scan_tmp_elems(size_t n) { return (n + SC_CHUNK - 1) / SC_CHUNK + 64; }
 
 __device__ __forceinline__ uint32_t block_exclusive_scan_256(uint32_t v, uint32_t* s_warp, uint32_t* block_total) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-        if (lane >= o) x += y;
-    }
+    const uint32_t x = warp_inclusive_scan(v);
     if (lane == 31) s_warp[warp] = x;
     __syncthreads();
     uint32_t off = 0, tot = 0;
@@ -662,8 +335,7 @@ __device__ __forceinline__ uint32_t block_exclusive_scan_256(uint32_t v, uint32_
     return off + x - v;
 }
 
-__global__ void __launch_bounds__(SC_THREADS) scan_reduce_kernel(const uint32_t* __restrict__ counts,
-                                                                 const uint32_t* __restrict__ perm, size_t n_cap,
+__global__ void __launch_bounds__(SC_THREADS) scan_reduce_kernel(const uint32_t* __restrict__ counts, size_t n_cap,
                                                                  const uint32_t* __restrict__ n_dev,
                                                                  uint32_t* __restrict__ partial) {
     __shared__ uint32_t s_warp[SC_THREADS / 32];
@@ -677,53 +349,14 @@ __global__ void __launch_bounds__(SC_THREADS) scan_reduce_kernel(const uint32_t*
 #pragma unroll
     for (int k = 0; k < SC_ITEMS; ++k) {
         const size_t i = base + (size_t)k * SC_THREADS + threadIdx.x;
-        if (i < n) sum += counts[perm ? perm[i] : i];
+        if (i < n) sum += counts[i];
     }
     uint32_t tot;
     block_exclusive_scan_256(sum, s_warp, &tot);
     if (threadIdx.x == 0) partial[blockIdx.x] = tot;
 }
 
-// single CTA: exclusive scan of the partials in place, grand total -> partial[m]
-__global__ void __launch_bounds__(1024) scan_partials_kernel(uint32_t* __restrict__ partial, uint32_t m) {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < m; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const uint32_t v = i < m ? partial[i] : 0u;
-        uint32_t x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t w = s_warp[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, w, o);
-                if (lane >= o) w += y;
-            }
-            s_warp[lane] = w;
-        }
-        __syncthreads();
-        const uint32_t warp_excl = warp == 0 ? 0u : s_warp[warp - 1];
-        const uint32_t carry = s_carry;
-        if (i < m) partial[i] = carry + warp_excl + x - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = carry + s_warp[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) partial[m] = s_carry;
-}
-
-__global__ void __launch_bounds__(SC_THREADS) scan_apply_kernel(const uint32_t* __restrict__ counts,
-                                                                const uint32_t* __restrict__ perm, size_t n_cap,
+__global__ void __launch_bounds__(SC_THREADS) scan_apply_kernel(const uint32_t* __restrict__ counts, size_t n_cap,
                                                                 const uint32_t* __restrict__ n_dev,
                                                                 const uint32_t* __restrict__ partial, uint32_t m,
                                                                 uint32_t* __restrict__ out, uint32_t* __restrict__ total_out) {
@@ -741,7 +374,7 @@ __global__ void __launch_bounds__(SC_THREADS) scan_apply_kernel(const uint32_t* 
 #pragma unroll
     for (int k = 0; k < SC_ITEMS; ++k) {
         const size_t i = base + k;
-        v[k] = i < n ? counts[perm ? perm[i] : i] : 0u;
+        v[k] = i < n ? counts[i] : 0u;
         sum += v[k];
     }
     uint32_t tot;
@@ -754,20 +387,20 @@ __global__ void __launch_bounds__(SC_THREADS) scan_apply_kernel(const uint32_t* 
     }
 }
 
-// out[i] = sum_{j<i} counts[perm[j]] for i < n, out[n] = total (also stored in *total_out); n = min(*n_dev, n_cap)
-int scan_gathered(const uint32_t* counts, const uint32_t* perm, uint32_t* out, size_t n_cap, uint32_t* tmp, cudaStream_t s,
-                  const uint32_t* n_dev, uint32_t* total_out) {
+// out[i] = sum_{j<i} counts[j] for i < n, out[n] = total (also stored in *total_out); n = min(*n_dev, n_cap)
+int exclusive_scan_u32(const uint32_t* counts, uint32_t* out, size_t n_cap, uint32_t* tmp, cudaStream_t s,
+                       const uint32_t* n_dev, uint32_t* total_out) {
     if (n_cap == 0) {
         GSR_CUDA(cudaMemsetAsync(out, 0, 4, s));
         if (total_out) GSR_CUDA(cudaMemsetAsync(total_out, 0, 4, s));
         return 0;
     }
     const uint32_t m = (uint32_t)((n_cap + SC_CHUNK - 1) / SC_CHUNK);
-    scan_reduce_kernel<<<m, SC_THREADS, 0, s>>>(counts, perm, n_cap, n_dev, tmp);
+    scan_reduce_kernel<<<m, SC_THREADS, 0, s>>>(counts, n_cap, n_dev, tmp);
     count_launches(1);
-    scan_partials_kernel<<<1, 1024, 0, s>>>(tmp, m);
+    rowscan_wide_kernel<1><<<1, 1024, 0, s>>>(tmp, m, tmp + m);     // the partials in place, grand total -> tmp[m]
     count_launches(1);
-    scan_apply_kernel<<<m, SC_THREADS, 0, s>>>(counts, perm, n_cap, n_dev, tmp, m, out, total_out);
+    scan_apply_kernel<<<m, SC_THREADS, 0, s>>>(counts, n_cap, n_dev, tmp, m, out, total_out);
     count_launches(1);
     GSR_CUDA(cudaGetLastError());
     return 0;

@@ -545,20 +545,6 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
     }
 }
 
-#ifndef GSR_BWD_PPT
-#define GSR_BWD_PPT 2     // default pixels per thread; GSR_BWD_PPT in the environment overrides (tuning aid)
-#endif
-
-static int bwd_ppt() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("GSR_BWD_PPT");
-        v = e ? atoi(e) : GSR_BWD_PPT;
-        if (v != 1 && v != 2 && v != 4) v = GSR_BWD_PPT;
-    }
-    return v;
-}
-
 int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, BwdAccum* accum, int ty0, int ty1, cudaStream_t s, const PeerAccum* peer,
                       unsigned char* touched) {
@@ -590,11 +576,7 @@ int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinSta
         count_launches(1);
         return 0;
     }
-    switch (bwd_ppt()) {
-        case 1: render_bwd_kernel<1><<<grid, PixelMap<1>::THREADS, 0, s>>>(p); break;
-        case 4: render_bwd_kernel<4><<<grid, PixelMap<4>::THREADS, 0, s>>>(p); break;
-        default: render_bwd_kernel<2><<<grid, PixelMap<2>::THREADS, 0, s>>>(p); break;
-    }
+    render_bwd_kernel<2><<<grid, PixelMap<2>::THREADS, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

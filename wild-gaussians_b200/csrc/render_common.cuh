@@ -29,25 +29,22 @@ __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
     return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
-// Thread -> pixel mapping inside a 16x16 tile.  A thread owns PPT pixels (1, 2 or 4) arranged PX x PY,
-// a warp owns a compact block of (8 PX) x (4 PY) pixels (the reference: one pixel per thread, a warp =
-// a 16x2 strip).  Per-pixel results do not depend on the mapping.  More pixels per thread amortise the
-// per-Gaussian shared-memory loads, loop control and (in the backward) the warp reduction over more
-// (pixel, Gaussian) pairs; the compact block keeps the per-warp culling selective and every 32-byte
-// output sector is written by one warp.
+// Thread -> pixel mapping inside a 16x16 tile.  A thread owns PPT vertically adjacent pixels (1 or 2), a warp owns a
+// compact block of 8 x (4 PPT) pixels (the reference: one pixel per thread, a warp = a 16x2 strip).  Per-pixel
+// results do not depend on the mapping.  Two pixels per thread amortise the per-Gaussian shared-memory loads, loop
+// control and (in the backward) the warp reduction over more (pixel, Gaussian) pairs; the compact block keeps the
+// per-warp culling selective and every 32-byte output sector is written by one warp.
 template <int PPT>
 struct PixelMap {
-    static_assert(PPT == 1 || PPT == 2 || PPT == 4, "PPT must be 1, 2 or 4");
-    static constexpr int PX = PPT == 4 ? 2 : 1;
-    static constexpr int PY = PPT >= 2 ? 2 : 1;
+    static_assert(PPT == 1 || PPT == 2, "PPT must be 1 or 2");
     static constexpr int THREADS = TILE * TILE / PPT;
     static constexpr int WARPS = THREADS / 32;
-    static constexpr int BW = 8 * PX, BH = 4 * PY;          // warp block in pixels
+    static constexpr int BW = 8, BH = 4 * PPT;          // warp block in pixels
     static constexpr int BLOCKS_X = TILE / BW;
     __device__ static __forceinline__ void pixel(int tid, int k, int& lx, int& ly) {
         const int warp = tid >> 5, lane = tid & 31;
-        lx = (warp % BLOCKS_X) * BW + (lane & 7) * PX + (k % PX);
-        ly = (warp / BLOCKS_X) * BH + (lane >> 3) * PY + (k / PX);
+        lx = (warp % BLOCKS_X) * BW + (lane & 7);
+        ly = (warp / BLOCKS_X) * BH + (lane >> 3) * PPT + k;
     }
 };
 

@@ -366,20 +366,6 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
     }
 }
 
-#ifndef GSR_FWD_PPT
-#define GSR_FWD_PPT 1     // default pixels per thread; GSR_FWD_PPT in the environment overrides (tuning aid)
-#endif
-
-static int fwd_ppt() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("GSR_FWD_PPT");
-        v = e ? atoi(e) : GSR_FWD_PPT;
-        if (v != 1 && v != 2 && v != 4) v = GSR_FWD_PPT;
-    }
-    return v;
-}
-
 int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, int ty0, int ty1, cudaStream_t s) {
     RenderFwdParams p;
@@ -401,11 +387,7 @@ int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinStat
         count_launches(1);
         return 0;
     }
-    switch (fwd_ppt()) {
-        case 1: render_fwd_kernel<1><<<grid, PixelMap<1>::THREADS, 0, s>>>(p); break;
-        case 4: render_fwd_kernel<4><<<grid, PixelMap<4>::THREADS, 0, s>>>(p); break;
-        default: render_fwd_kernel<2><<<grid, PixelMap<2>::THREADS, 0, s>>>(p); break;
-    }
+    render_fwd_kernel<1><<<grid, PixelMap<1>::THREADS, 0, s>>>(p);
     count_launches(1);
     return 0;
 }
