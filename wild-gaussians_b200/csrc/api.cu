@@ -100,6 +100,7 @@ size_t carve_img(char* base, int W, int H, ImgState* out) {
     take(cur, im.final_T, N, 128);   // first 128-B aligned field, like the reference ImageState
     take(cur, im.n_contrib, N);
     take(cur, im.ranges, T);
+    take(cur, im.blend_mask, T * MASK_BLOCKS * MASK_WORDS);
     if (out) *out = im;
     return (size_t)(cur - base) + 256;
 }

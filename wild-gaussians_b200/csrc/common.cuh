@@ -69,10 +69,20 @@ struct GeomState {
     uint32_t* radix_tmp;      // histogram / scan temporaries
 };
 
+// Blend masks: the forward records, for each tile, each 8x8 pixel block of the tile (in the packed kernels' warp
+// order: block k covers pixels [8 (k % 2), +8) x [8 (k / 2), +8)) and each of the first MASK_K positions of the
+// tile's list, whether some pixel of the block blended that position.  Bit b of word w is position 32 w + b.  The
+// backward walks only the set bits; positions at or above MASK_K are culled by the footprint box instead.
+constexpr int MASK_K = 1024;
+constexpr int MASK_WORDS = MASK_K / 32;   // words per (tile, block)
+constexpr int MASK_BLOCKS = 4;            // 8x8 blocks per tile
+
 struct ImgState {
     float*    final_T;        // [N]  first, 128-B aligned (reference ImageState order)
     uint32_t* n_contrib;      // [N]
     uint2*    ranges;         // [T]
+    uint32_t* blend_mask;     // [T][MASK_BLOCKS][MASK_WORDS]; only the words below the block's largest n_contrib are
+                              // defined (the forward walked those batches with some pixel of the block compositing)
 };
 
 struct BinState {

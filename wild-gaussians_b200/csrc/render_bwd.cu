@@ -7,14 +7,18 @@
 // issues 10 global float atomics per blended (pixel, Gaussian) pair (backward.cu:568-603).
 // Here all 32 lanes of a warp walk the same Gaussian in lock-step, so the 10 per-lane terms
 // are summed across the warp with a multi-value shuffle butterfly (12 shuffles instead of
-// 50), then added to a per-tile shared-memory accumulator (one shared atomic per component
-// per warp), and a tile writes each visited Gaussian's 10 sums to HBM once, as three
+// 50), stored into the warp's private row of the staged Gaussian (PartRows), and a tile adds
+// the rows in warp order and writes each visited Gaussian's 10 sums to HBM once, as three
 // 128-bit vector reductions (red.global.add.v4.f32) into a packed 48-byte record.
 // That is up to 256x fewer L2 atomics per Gaussian per tile.
 //
 // The walk starts at the tile's largest n_contrib instead of the end of the tile's range:
 // instances behind every pixel's last contributor are skipped by the reference one by one
-// (backward.cu:531-533); skipping them wholesale gives the same sums.
+// (backward.cu:531-533); skipping them wholesale gives the same sums.  Below MASK_K a warp
+// walks only the positions the forward's blend mask marks for its 8x8 block (common.cuh):
+// for a pixel, "blends at position i in the backward" (i < n_contrib, power <= 0,
+// alpha >= 1/255) is exactly "updated at position i in the forward", so no walked step is
+// wasted.  Beyond MASK_K the footprint box culls as before.
 //
 // The |grad| channel (backward.cu:593-595) is the sum over pixels of |gx| + |gy|, so the
 // absolute value is taken per lane BEFORE the warp reduction.
@@ -45,7 +49,33 @@ struct RenderBwdParams {
     int n_peers;
     float* mc;             // multicast address of the same symmetric buffer, or NULL
     unsigned char* touched;   // pull-mode reduction: touched[g] = 1 for every Gaussian this rank added to, or NULL
+    const uint32_t* blend_mask;   // written by the forward (common.cuh)
 };
+
+// Stage the blend-mask words a round needs: for each warp (= 8x8 block k), the NW words from word w_lo on.  Words at or
+// above the block's largest n_contrib were possibly never written by the forward, and words at or above MASK_WORDS do
+// not exist: both read as 0 (their positions are culled by `pos < warp_last` or by the footprint box).
+template <int WARPS, int NW>
+__device__ __forceinline__ void stage_mask_words(const RenderBwdParams& p, int tile, int w_lo, const uint32_t* s_max,
+                                                 uint32_t (*s_mask)[NW]) {
+    const int tid = threadIdx.x;
+    if (tid < WARPS * NW) {
+        const int k = tid / NW, word = w_lo + tid % NW;
+        uint32_t m = 0;
+        if (word < MASK_WORDS && 32 * word < (int)s_max[k]) m = p.blend_mask[((size_t)tile * MASK_BLOCKS + k) * MASK_WORDS + word];
+        s_mask[k][tid % NW] = m;
+    }
+}
+
+// Does the warp walk staged entry jl of the round (list position pos = first_pos - jl)?  Below MASK_K: exactly when the
+// forward blended that position in some pixel of the warp's block.  Above: when the footprint can reach alpha >= 1/255
+// in the block (box, then ellipse; render_common.cuh).  con = {conic.x, conic.y, conic.z, opacity}.
+__device__ __forceinline__ bool bwd_walks(int pos, uint32_t warp_last, int w_lo, const uint32_t* mask_words, const float4 geo,
+                                          const float4 con, const WarpBox& box) {
+    if ((uint32_t)pos >= warp_last) return false;
+    if (pos < MASK_K) return (mask_words[(pos >> 5) - w_lo] >> (pos & 31)) & 1u;
+    return box_may_touch(geo, box) && ellipse_may_touch(geo.x, geo.y, con.x, con.y, con.z, con.w, box);
+}
 
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
@@ -122,6 +152,34 @@ __device__ __forceinline__ int butterfly10(float (&v)[10], int lane) {
     return idx < 0 ? 15 : idx + 5 * b4;
 }
 
+// Per-warp private accumulator rows.  A warp visits a staged Gaussian at most once per round, so its butterfly sums go
+// to its own row s_part[warp][slot] with plain stores (no shared-memory atomics, which sm_90 runs as a compare-and-swap
+// loop), and bit slot of s_wrote[warp] records that the row holds this round's sums.  The flush adds the written rows
+// of a slot in warp order, so the in-tile summation order is fixed.
+template <int WARPS, int RB>
+struct PartRows {
+    float4 row[WARPS][RB][RB_ACC / 4];
+    uint32_t wrote[WARPS][RB / 32];
+    // sum of slot j's written rows into (a0, a1, a2); false if no warp wrote one.  One float4 column at a time, so that
+    // few registers are live next to the per-pixel state.
+    __device__ __forceinline__ bool sum(int j, float4& a0, float4& a1, float4& a2) const {
+        unsigned writers = 0;
+#pragma unroll
+        for (int k = 0; k < WARPS; ++k) writers |= ((wrote[k][j >> 5] >> (j & 31)) & 1u) << k;
+        a0 = column(j, 0, writers); a1 = column(j, 1, writers); a2 = column(j, 2, writers);
+        return writers != 0;
+    }
+    __device__ __forceinline__ float4 column(int j, int c, unsigned writers) const {
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+        for (; writers; writers &= writers - 1) {
+            const float4 b = row[__ffs(writers) - 1][j][c];
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        return a;
+    }
+};
+
 __device__ __forceinline__ float rcp_approx(float x) {
     float r;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -141,12 +199,17 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
     using PM = PixelMap<PPT>;
     constexpr int THREADS = PM::THREADS;
     constexpr int WARPS = PM::WARPS;
-    __shared__ uint32_t s_id[RT_BATCH];
-    __shared__ __align__(16) float4 s_geo[RT_BATCH];   // {x, y, hx, hy}
-    __shared__ __align__(16) float4 s_con[RT_BATCH];   // {conic.x, conic.y, conic.z, opacity}
-    __shared__ __align__(16) float4 s_col[RT_BATCH];   // {r, g, b, -}
-    __shared__ __align__(16) float s_acc[RT_BATCH][RB_ACC];
+    constexpr int RB = 64;   // instances staged per round: four private rows of 64 slots keep the shared memory small
+    static_assert(RB <= THREADS, "one staged instance per thread");
+    __shared__ uint32_t s_id[RB];
+    __shared__ __align__(16) float4 s_geo[RB];   // {x, y, hx, hy}
+    __shared__ __align__(16) float4 s_con[RB];   // {conic.x, conic.y, conic.z, opacity}
+    __shared__ __align__(16) float4 s_col[RB];   // {r, g, b, -}
+    __shared__ PartRows<WARPS, RB> s_part;
     __shared__ uint32_t s_max[WARPS];
+    constexpr int NW = RB / 32 + 1;   // mask words a round's positions can span
+    __shared__ uint32_t s_mask[WARPS][NW];
+    static_assert(WARPS == MASK_BLOCKS, "one warp per 8x8 blend-mask block");
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
@@ -200,7 +263,7 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
 #pragma unroll
     for (int w = 0; w < WARPS; ++w) tile_last = max(tile_last, s_max[w]);
     const int total = (int)min(tile_last, range.y - range.x);   // instances [range.x, range.x+total) matter
-    const int rounds = (total + RT_BATCH - 1) / RT_BATCH;
+    const int rounds = (total + RB - 1) / RB;
 
     // Gradient of pixel coordinate w.r.t. normalized screen-space viewport coordinates (-1 to 1)
     const float ddelx_dx = 0.5f * p.W;
@@ -217,37 +280,31 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
     const bool slot_owner = (lane & 1) == 0 && my_slot < 10;
 
     int toDo = total;
-    for (int r = 0; r < rounds; ++r, toDo -= RT_BATCH) {
-        __syncthreads();   // previous round's accumulators flushed, staging buffers free
-#pragma unroll
-        for (int q = 0; q < PPT; ++q) {
-            const int slot = q * THREADS + tid;
-            const int progress = r * RT_BATCH + slot;
-            if (progress < total) {
-                const uint32_t id = p.point_list[range.x + total - progress - 1];
-                s_id[slot] = id;
-                const float4* src = p.rec + 2 * (size_t)id;
-                s_geo[slot] = src[0];
-                s_con[slot] = src[1];
-                const float* c = p.colors + 3 * (size_t)id;
-                s_col[slot] = make_float4(c[0], c[1], c[2], 0.f);
-            }
-            float4* a = reinterpret_cast<float4*>(s_acc[slot]);
-            a[0] = a[1] = a[2] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int r = 0; r < rounds; ++r, toDo -= RB) {
+        const int n = min(RB, toDo);
+        // 0-based list position of staged entry j: pos(j) = first_pos - j  (walking back to front)
+        const int first_pos = total - 1 - r * RB;
+        const int w_lo = (first_pos - n + 1) >> 5;
+        __syncthreads();   // previous round's rows flushed, staging buffers free
+        stage_mask_words<WARPS, NW>(p, tile_y * p.grid_x + tile_x, w_lo, s_max, s_mask);
+        if (tid < n) {
+            const uint32_t id = p.point_list[range.x + first_pos - tid];
+            s_id[tid] = id;
+            const float4* src = p.rec + 2 * (size_t)id;
+            s_geo[tid] = src[0];
+            s_con[tid] = src[1];
+            const float* c = p.colors + 3 * (size_t)id;
+            s_col[tid] = make_float4(c[0], c[1], c[2], 0.f);
         }
         __syncthreads();
 
-        const int n = min(RT_BATCH, toDo);
-        // 0-based list position of staged entry j: pos(j) = first_pos - j  (walking back to front)
-        const int first_pos = total - 1 - r * RT_BATCH;
-
 #pragma unroll 1
-        for (int w = 0; w < RT_BATCH / 32; ++w) {
-            // per-warp culling: staged Gaussians that are in front of this warp's deepest contributor and whose
-            // alpha >= 1/255 footprint can touch the warp's pixel block
+        for (int w = 0; w < RB / 32; ++w) {
+            // per-warp culling: the positions the forward blended in this warp's block (bwd_walks)
             const int jl = w * 32 + lane;
-            const bool rel = jl < n && (uint32_t)(first_pos - jl) < warp_last && box_may_touch(s_geo[jl], box);
+            const bool rel = jl < n && bwd_walks(first_pos - jl, warp_last, w_lo, s_mask[warp], s_geo[jl], s_con[jl], box);
             unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
+            uint32_t wrote = 0;
             while (mm) {
                 const int j = w * 32 + __ffs(mm) - 1;
                 mm &= mm - 1;
@@ -276,7 +333,8 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
                     alpha[k] = act ? a : 0.f;
                     any_active |= act;
                 }
-                if (!__any_sync(0xFFFFFFFFu, any_active)) continue;   // warp-uniform
+                // below MASK_K some pixel of the warp blends by construction; above, the box test is only conservative
+                if (pos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, any_active)) continue;   // warp-uniform
 
                 const float4 col = s_col[j];
                 const float kx = fabsf(con_o.w) * ddelx_dx, ky = fabsf(con_o.w) * ddely_dy;
@@ -312,31 +370,26 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(cons
                     }
                 }
                 butterfly10(v, lane);
-                if (slot_owner) atomicAdd(&s_acc[j][my_slot], v[0]);
+                if (slot_owner) reinterpret_cast<float*>(s_part.row[warp][j])[my_slot] = v[0];
+                wrote |= 1u << (j - w * 32);
             }
+            if (lane == 0) s_part.wrote[warp][w] = wrote;
         }
         __syncthreads();
         // one flush per visited Gaussian per tile: moments -> gradient terms, three 128-bit reductions
         // (skipped when nothing landed)
-#pragma unroll
-        for (int q = 0; q < PPT; ++q) {
-            const int slot = q * THREADS + tid;
-            if (slot < n) {
-                const float* a = s_acc[slot];
-                const float4 a0 = *reinterpret_cast<const float4*>(a);
-                const float4 a1 = *reinterpret_cast<const float4*>(a + 4);
-                const float4 a2 = *reinterpret_cast<const float4*>(a + 8);
-                const bool any = (a0.x != 0.f) | (a0.y != 0.f) | (a0.z != 0.f) | (a0.w != 0.f) | (a1.x != 0.f) |
-                                 (a1.y != 0.f) | (a1.z != 0.f) | (a1.w != 0.f) | (a2.x != 0.f) | (a2.y != 0.f);
-                if (any) {
-                    const float4 con_o = s_con[slot];
-                    const float o = con_o.w;
-                    const float gx = -o * ddelx_dx * (con_o.x * a0.x + con_o.y * a0.y);
-                    const float gy = -o * ddely_dy * (con_o.z * a0.y + con_o.y * a0.x);
-                    const float h = -0.5f * o;
-                    flush_row<false>(p, s_id[slot], make_float4(gx, gy, a0.z, h * a0.w), make_float4(h * a1.x, h * a1.y, a1.z, a1.w),
-                              make_float4(a2.x, a2.y, 0.f, 0.f));
-                }
+        float4 a0, a1, a2;
+        if (tid < n && s_part.sum(tid, a0, a1, a2)) {
+            const bool any = (a0.x != 0.f) | (a0.y != 0.f) | (a0.z != 0.f) | (a0.w != 0.f) | (a1.x != 0.f) |
+                             (a1.y != 0.f) | (a1.z != 0.f) | (a1.w != 0.f) | (a2.x != 0.f) | (a2.y != 0.f);
+            if (any) {
+                const float4 con_o = s_con[tid];
+                const float o = con_o.w;
+                const float gx = -o * ddelx_dx * (con_o.x * a0.x + con_o.y * a0.y);
+                const float gy = -o * ddely_dy * (con_o.z * a0.y + con_o.y * a0.x);
+                const float h = -0.5f * o;
+                flush_row<false>(p, s_id[tid], make_float4(gx, gy, a0.z, h * a0.w), make_float4(h * a1.x, h * a1.y, a1.z, a1.w),
+                          make_float4(a2.x, a2.y, 0.f, 0.f));
             }
         }
     }
@@ -359,17 +412,20 @@ struct __align__(16) PairRec {      // 80 bytes per staged Gaussian
 __device__ __forceinline__ float2 lo2(const float4 v) { return make_float2(v.x, v.y); }
 __device__ __forceinline__ float2 hi2(const float4 v) { return make_float2(v.z, v.w); }
 
+// (128, 9): at most 56 registers, so that 9 CTAs (36 warps) fit an SM, as the shared memory allows
 template <bool PEER>
-__global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_constant__ RenderBwdParams p) {
+__global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_constant__ RenderBwdParams p) {
     using PM = PixelMap<2>;
     constexpr int THREADS = PM::THREADS;   // 128
     constexpr int WARPS = PM::WARPS;       // 4
-    constexpr int PB = 128;                // instances staged per round (one per thread)
+    constexpr int PB = 64;                 // instances staged per round: four private rows of 64 slots keep 9 CTAs/SM
     __shared__ uint32_t s_id[PB];
     __shared__ __align__(16) float4 s_geo[PB];    // {x, y, hx, hy} for the per-warp culling
     __shared__ PairRec s_rec[PB];
-    __shared__ __align__(16) float s_acc[PB][RB_ACC];
+    __shared__ PartRows<WARPS, PB> s_part;
     __shared__ uint32_t s_max[WARPS];
+    constexpr int NW = PB / 32 + 1;
+    __shared__ uint32_t s_mask[WARPS][NW];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
@@ -434,11 +490,14 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
 
     int toDo = total;
     for (int r = 0; r < rounds; ++r, toDo -= PB) {
+        const int n = min(PB, toDo);
+        const int first_pos = total - 1 - r * PB;
+        const int w_lo = (first_pos - n + 1) >> 5;
         __syncthreads();
+        stage_mask_words<WARPS, NW>(p, tile_y * p.grid_x + tile_x, w_lo, s_max, s_mask);
         {
-            const int progress = r * PB + tid;
-            if (progress < total) {
-                const uint32_t id = p.point_list[range.x + total - progress - 1];
+            if (tid < n) {
+                const uint32_t id = p.point_list[range.x + first_pos - tid];
                 s_id[tid] = id;
                 const float4* src = p.rec + 2 * (size_t)id;
                 const float4 g = src[0], c = src[1];
@@ -453,19 +512,16 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
                 rec.bk = make_float4(cb, cb, fabsf(c.w) * ddelx_dx, fabsf(c.w) * ddely_dy);
                 s_rec[tid] = rec;
             }
-            float4* a = reinterpret_cast<float4*>(s_acc[tid]);
-            a[0] = a[1] = a[2] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         __syncthreads();
-
-        const int n = min(PB, toDo);
-        const int first_pos = total - 1 - r * PB;
 
 #pragma unroll 1
         for (int w = 0; w < PB / 32; ++w) {
             const int jl = w * 32 + lane;
-            const bool rel = jl < n && (uint32_t)(first_pos - jl) < warp_last && box_may_touch(s_geo[jl], box);
+            const bool rel = jl < n && bwd_walks(first_pos - jl, warp_last, w_lo, s_mask[warp], s_geo[jl],
+                                                 make_float4(s_rec[jl].ac.x, -s_rec[jl].bo.x, s_rec[jl].ac.z, s_rec[jl].bo.z), box);
             unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
+            uint32_t wrote = 0;
             while (mm) {
                 const int j = w * 32 + __ffs(mm) - 1;
                 mm &= mm - 1;
@@ -485,7 +541,7 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
                 const float a0 = min(0.99f, oG.x), a1 = min(0.99f, oG.y);
                 const bool act0 = pos < last_contributor[0] && !(power.x > 0.0f) && !(a0 < 1.0f / 255.0f);
                 const bool act1 = pos < last_contributor[1] && !(power.y > 0.0f) && !(a1 < 1.0f / 255.0f);
-                if (!__any_sync(0xFFFFFFFFu, act0 || act1)) continue;   // warp-uniform
+                if (pos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, act0 || act1)) continue;   // see the scalar kernel
                 // pairs that do not blend run through the arithmetic as G = alpha = 0 (see the scalar kernel)
                 const float2 G = make_float2(act0 ? g0 : 0.f, act1 ? g1 : 0.f);
                 const float2 alpha = make_float2(act0 ? a0 : 0.f, act1 ? a1 : 0.f);
@@ -521,15 +577,14 @@ __global__ void __launch_bounds__(128) render_bwd_packed_kernel(const __grid_con
                 v[8] = c1.x + c1.y;
                 v[9] = c2.x + c2.y;
                 butterfly10(v, lane);
-                if (slot_owner) atomicAdd(&s_acc[j][my_slot], v[0]);
+                if (slot_owner) reinterpret_cast<float*>(s_part.row[warp][j])[my_slot] = v[0];
+                wrote |= 1u << (j - w * 32);
             }
+            if (lane == 0) s_part.wrote[warp][w] = wrote;
         }
         __syncthreads();
-        if (tid < n) {
-            const float* a = s_acc[tid];
-            const float4 a0 = *reinterpret_cast<const float4*>(a);
-            const float4 a1 = *reinterpret_cast<const float4*>(a + 4);
-            const float4 a2 = *reinterpret_cast<const float4*>(a + 8);
+        float4 a0, a1, a2;
+        if (tid < n && s_part.sum(tid, a0, a1, a2)) {
             const bool any = (a0.x != 0.f) | (a0.y != 0.f) | (a0.z != 0.f) | (a0.w != 0.f) | (a1.x != 0.f) |
                              (a1.y != 0.f) | (a1.z != 0.f) | (a1.w != 0.f) | (a2.x != 0.f) | (a2.y != 0.f);
             if (any) {
@@ -557,7 +612,7 @@ int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinSta
     p.ranges = im.ranges; p.point_list = b.point_list;
     p.subpixel_offset = reinterpret_cast<const float2*>(a.subpixel_offset);
     p.bg = a.background; p.rec = g.rec; p.colors = colors;
-    p.final_T = im.final_T; p.n_contrib = im.n_contrib; p.dL_dpix = a.dL_dpix;
+    p.final_T = im.final_T; p.n_contrib = im.n_contrib; p.dL_dpix = a.dL_dpix; p.blend_mask = im.blend_mask;
     p.accum = reinterpret_cast<float*>(accum);
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);

@@ -69,4 +69,25 @@ __device__ __forceinline__ bool box_may_touch(const float4 g, const WarpBox& b) 
     return !(g.z < 0.f || g.x + g.z < b.x0 || g.x - g.z > b.x1 || g.y + g.w < b.y0 || g.y - g.w > b.y1);
 }
 
+// Can the Gaussian with centre (x, y), conic (A, B, C) and opacity o reach alpha >= 1/255 at some sample of the box?
+// With u = x - px, v = y - py the kernels' power is -q/2, q = A u^2 + 2 B u v + C v^2, and alpha >= 1/255 needs
+// q <= 2 ln(255 o).  The minimum of q over the box is 0 if the centre is inside; otherwise it lies on the boundary
+// (q is a convex 1-D quadratic along every edge since A, C > 0, and has no interior minimum off the centre), so it is
+// the least of the four clamped 1-D edge minima.  Conservative like the extents (preprocess_fwd.cu): every q is
+// lowered by 1e-3 of the magnitude of its terms and the bound raised by 2e-3, far above fp32 rounding and the error
+// of __logf; a non-positive A or C, or a NaN, keeps the Gaussian.  Use after box_may_touch (negative extents).
+__device__ __forceinline__ bool ellipse_may_touch(float x, float y, float A, float B, float C, float o, const WarpBox& b) {
+    const float u0 = x - b.x1, u1 = x - b.x0, v0 = y - b.y1, v1 = y - b.y0;
+    if (u0 <= 0.f && u1 >= 0.f && v0 <= 0.f && v1 >= 0.f) return true;
+    if (!(A > 0.f && C > 0.f)) return true;
+    const float rA = __frcp_rn(A), rC = __frcp_rn(C);
+    auto q_lo = [&](float u, float v) {
+        const float a = A * u * u, c = C * v * v, m = 2.f * B * u * v;
+        return (a + c + m) - 1e-3f * (a + c + fabsf(m));
+    };
+    const float q = fminf(fminf(q_lo(u0, fminf(fmaxf(-B * u0 * rC, v0), v1)), q_lo(u1, fminf(fmaxf(-B * u1 * rC, v0), v1))),
+                          fminf(q_lo(fminf(fmaxf(-B * v0 * rA, u0), u1), v0), q_lo(fminf(fmaxf(-B * v1 * rA, u0), u1), v1)));
+    return !(q > 2.f * __logf(255.f * o) + 2e-3f);
+}
+
 }  // namespace gsr

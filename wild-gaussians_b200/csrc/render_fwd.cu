@@ -10,10 +10,15 @@
 //
 // Per-warp culling: before blending a round, every lane tests 8 of the 256 staged Gaussians against the
 // bounding box of the warp's sample positions using the conservative footprint extents computed in
-// preprocess_fwd.cu; eight ballots give the warp a 256-bit mask and only the set bits are blended.
+// preprocess_fwd.cu, then against the footprint ellipse itself (ellipse_may_touch, render_common.cuh);
+// eight ballots give the warp a 256-bit mask and only the set bits are blended.
 // The skipped (pixel, Gaussian) pairs are pairs the reference rejects with alpha < 1/255
 // (forward.cu:365), so the image, final_T and n_contrib are unchanged; `contributor` is derived from
 // the position in the list, not counted, so it still counts every instance like forward.cu:349.
+//
+// Blend masks: for the first MASK_K positions of a tile's list, every kernel records per 8x8 pixel
+// block whether some pixel of the block blended the position (common.cuh).  The backward walks only
+// those positions.
 //
 // Numerics contract (SURVEY.md 8a note N3): the expression shapes of power / alpha / test_T / the
 // colour accumulation are exactly the reference's (forward.cu:353-378,393), and expf is the accurate
@@ -35,21 +40,30 @@ struct RenderFwdParams {
     float* final_T;
     uint32_t* n_contrib;
     float* out_color;
+    uint32_t* blend_mask;      // [T][MASK_BLOCKS][MASK_WORDS] (common.cuh)
     // multi-GPU: the band is stored into the [4,H,W] images (colour + final transmittance) of ALL ranks through
     // peer-mapped pointers (image all-gather fused into the composite's epilogue); NULL / 0 = local out_color only
     float* const* peer_out;
     int n_peers;
 };
 
+// word `word` of 8x8 block k of this CTA's tile
+__device__ __forceinline__ uint32_t* blend_mask_word(const RenderFwdParams& p, int k, int word) {
+    const int tile = (blockIdx.y + p.ty0) * p.grid_x + blockIdx.x;
+    return p.blend_mask + ((size_t)tile * MASK_BLOCKS + k) * MASK_WORDS + word;
+}
+
 template <int PPT>
 __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_fwd_kernel(const __grid_constant__ RenderFwdParams p) {
     using PM = PixelMap<PPT>;
+    static_assert(PPT == 1, "the blend-mask combine below assumes 8 warps of 8x4 pixels");
     constexpr int THREADS = PM::THREADS;
     __shared__ __align__(16) float4 s_geo[2][RT_BATCH];   // {x, y, hx, hy}
     __shared__ __align__(16) float4 s_con[2][RT_BATCH];   // {conic.x, conic.y, conic.z, opacity}
     __shared__ __align__(16) float4 s_col[2][RT_BATCH];   // {r, g, b, -}
+    __shared__ uint32_t s_blend[PM::WARPS][RT_BATCH / 32];   // this round's blend-mask words of each warp
 
-    const int tid = threadIdx.x, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
 
     float2 pixf[PPT];
@@ -134,18 +148,26 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_fwd_kernel(cons
 
             const int n = min(RT_BATCH, toDo);
             const uint32_t round_base = (uint32_t)(r * RT_BATCH);
+            uint32_t my_word = 0;   // lane w holds the blend-mask word of the round's batch w
             if (__any_sync(0xFFFFFFFFu, live != 0)) {
                 // which of the staged Gaussians can touch this warp's pixels?  32 at a time: one ballot, then only
                 // the set bits are blended
 #pragma unroll 1
                 for (int w = 0; w < RT_BATCH / 32; ++w) {
                     const int jl = w * 32 + lane;
-                    unsigned mm = __ballot_sync(0xFFFFFFFFu, jl < n && box_may_touch(s_geo[buf][jl], box));
+                    bool rel = false;
+                    if (jl < n) {
+                        const float4 g = s_geo[buf][jl], c = s_con[buf][jl];
+                        rel = box_may_touch(g, box) && ellipse_may_touch(g.x, g.y, c.x, c.y, c.z, c.w, box);
+                    }
+                    unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
+                    uint32_t blended = 0;
                     while (mm) {
                         const int j = w * 32 + __ffs(mm) - 1;
                         mm &= mm - 1;
                         const float4 geo = s_geo[buf][j];
                         const float4 con_o = s_con[buf][j];
+                        bool upd = false;
 #pragma unroll
                         for (int k = 0; k < PPT; ++k) {
                             if (!(live & (1u << k))) continue;
@@ -168,13 +190,25 @@ __global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_fwd_kernel(cons
                             T[k] = test_T;
                             // 1-based position of this instance in the tile's list (forward.cu:349,382)
                             last_contributor[k] = round_base + (uint32_t)j + 1u;
+                            upd = true;
                         }
+                        if (__any_sync(0xFFFFFFFFu, upd)) blended |= 1u << (j - w * 32);
                     }
+                    if (lane == w) my_word = blended;
                     if (!__any_sync(0xFFFFFFFFu, live != 0)) break;
                 }
             }
+            if (lane < RT_BATCH / 32) s_blend[warp][lane] = my_word;
             // everyone is finished with `buf` before round r+2 is staged into it
             __syncthreads();
+            // an 8x8 block is two 8x4 warp blocks (warps wa and wa + 2): its words are the OR of theirs.  s_blend is
+            // rewritten only after the next round's barrier.
+            if (tid < MASK_BLOCKS * (RT_BATCH / 32)) {
+                const int k = tid / (RT_BATCH / 32), i = tid % (RT_BATCH / 32);
+                const int wa = (k & 1) + 4 * (k >> 1);
+                const int word = r * (RT_BATCH / 32) + i;
+                if (word < MASK_WORDS) *blend_mask_word(p, k, word) = s_blend[wa][i] | s_blend[wa + 2][i];
+            }
         }
         cp_async_wait<0>();
     }
@@ -207,15 +241,16 @@ struct __align__(16) FwdPairRec {     // 80 bytes
     float4 ac;     // {conic.x, conic.x, conic.z, conic.z}
     float4 bo;     // {-conic.y, -conic.y, opacity, opacity}
     float4 rg;     // {r, r, g, g}
-    float4 bb;     // {b, b, -, -}
+    float4 bb;     // {b, b, hx, hy}: the footprint extents for the per-warp culling
 };
 
-__global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_constant__ RenderFwdParams p) {
+// (128, 9): at most 56 registers, so that 9 CTAs (36 warps) fit an SM, as the shared memory allows
+__global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_constant__ RenderFwdParams p) {
     using PM = PixelMap<2>;
     constexpr int THREADS = 128;
     constexpr int PB = 128;               // instances per round
-    __shared__ __align__(16) float4 s_geo[2][PB];      // {x, y, hx, hy} for the per-warp culling
     __shared__ FwdPairRec s_rec[2][PB];
+    __shared__ uint32_t s_blend[PixelMap<2>::WARPS][MASK_WORDS];   // blend-mask words, written out at the end
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
@@ -279,14 +314,13 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
         for (int r = 0; r < rounds; ++r, toDo -= PB) {
             const int buf = r & 1;
             // write this round's (already loaded) record, duplicated, then start the next round's loads
-            s_geo[buf][tid] = g;
             {
                 FwdPairRec rec;
                 rec.xy = make_float4(g.x, g.x, g.y, g.y);
                 rec.ac = make_float4(c.x, c.x, c.z, c.z);
                 rec.bo = make_float4(-c.y, -c.y, c.w, c.w);
                 rec.rg = make_float4(cr, cr, cg, cg);
-                rec.bb = make_float4(cb, cb, 0.f, 0.f);
+                rec.bb = make_float4(cb, cb, g.z, g.w);
                 s_rec[buf][tid] = rec;
             }
             if (r + 1 < rounds) {
@@ -304,7 +338,14 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
 #pragma unroll 1
                 for (int w = 0; w < PB / 32; ++w) {
                     const int jl = w * 32 + lane;
-                    unsigned mm = __ballot_sync(0xFFFFFFFFu, jl < n && box_may_touch(s_geo[buf][jl], box));
+                    bool rel = false;
+                    if (jl < n) {
+                        const FwdPairRec& L = s_rec[buf][jl];
+                        rel = box_may_touch(make_float4(L.xy.x, L.xy.z, L.bb.z, L.bb.w), box) &&
+                              ellipse_may_touch(L.xy.x, L.xy.z, L.ac.x, -L.bo.x, L.ac.z, L.bo.z, box);
+                    }
+                    unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
+                    uint32_t blended = 0;   // bit b: some pixel of the warp blended position round_base + 32 w + b
                     while (mm) {
                         const int j = w * 32 + __ffs(mm) - 1;
                         mm &= mm - 1;
@@ -325,6 +366,7 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
                         live1 = live1 && !stop1;
                         const bool upd0 = blend0 && !stop0, upd1 = blend1 && !stop1;
                         if (!__any_sync(0xFFFFFFFFu, upd0 || upd1)) continue;
+                        blended |= 1u << (j - w * 32);
                         const float2 alpha = make_float2(upd0 ? a0 : 0.f, upd1 ? a1 : 0.f);
                         const float4 rg = R.rg, bb = R.bb;
                         C0 = fma2(T, mul2(alpha, make_float2(rg.x, rg.y)), C0);
@@ -336,11 +378,18 @@ __global__ void __launch_bounds__(128) render_fwd_packed_kernel(const __grid_con
                         last0 = upd0 ? idx : last0;
                         last1 = upd1 ? idx : last1;
                     }
+                    const int word = (int)(round_base / 32) + w;
+                    if (lane == 0 && word < MASK_WORDS) s_blend[tid >> 5][word] = blended;
                     if (!__any_sync(0xFFFFFFFFu, live0 || live1)) break;
                 }
             }
         }
     }
+
+    // PixelMap<2>: warp k is 8x8 block k.  Words of batches no warp entered are copied too; they are never read.
+    __syncthreads();
+    for (int i = tid; i < MASK_BLOCKS * MASK_WORDS; i += THREADS)
+        *blend_mask_word(p, i / MASK_WORDS, i % MASK_WORDS) = s_blend[i / MASK_WORDS][i % MASK_WORDS];
 
     const size_t plane = (size_t)p.H * p.W;
     const float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
@@ -373,7 +422,7 @@ int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinStat
     p.ranges = im.ranges; p.point_list = b.point_list;
     p.subpixel_offset = reinterpret_cast<const float2*>(a.subpixel_offset);
     p.rec = g.rec; p.colors = colors; p.bg = a.background;
-    p.final_T = im.final_T; p.n_contrib = im.n_contrib; p.out_color = a.out_color;
+    p.final_T = im.final_T; p.n_contrib = im.n_contrib; p.out_color = a.out_color; p.blend_mask = im.blend_mask;
     p.peer_out = (float* const*)(a.peer_images); p.n_peers = a.n_peer_images;
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);
