@@ -354,6 +354,18 @@ int gsr_compute_3d_filter(int P, const float* xyz, int num_cameras, const float*
 size_t gsr_knn_scratch_bytes(int P);
 int gsr_knn_mean_dist2(int P, const float* points, float* mean_dist2, void* scratch, void* stream);
 
+/* -- SSIM of the photometric loss (optional entry points) ---------------------------------------------------------------
+ * The `ssim` of wildgaussians/method.py:644-673 (11-tap Gaussian window, sigma 1.5, zero padding 5, C1 = 0.01^2,
+ * C2 = 0.03^2; map = mean over the 3 channels of the per-channel SSIM), one kernel per direction.  img1, img2:
+ * [B,3,H,W] fp32, contiguous, on the device; ssim_map: [B,H,W].  partials: NULL when no backward follows, otherwise
+ * [B][3 factors][3 channels][H][W] fp32 (36 B per pixel: dS/dmu_x, dS/dE_xx, dS/dE_xy per channel), written by the
+ * forward and read by the backward.  The backward takes the upstream dL_dmap [B,H,W] and writes dL_dimg1 [B,3,H,W]
+ * (no gradient for img2).  B <= 65535.                                                                                    */
+int gsr_ssim_forward(int B, int H, int W, const float* img1, const float* img2, float* ssim_map, float* partials /* NULL: no backward */,
+                     void* stream);
+int gsr_ssim_backward(int B, int H, int W, const float* img1, const float* img2, const float* partials, const float* dL_dmap,
+                      float* dL_dimg1, void* stream);
+
 /* Optional per-stage device timing (cudaEvents on the caller's stream around each stage of the
  * next forward / backward calls).  The caller synchronises the stream, then reads the stage times of
  * the most recent calls in milliseconds (-1 for stages that did not run).  Not thread-safe.        */

@@ -127,6 +127,10 @@ def _load():
     lib.gsr_knn_scratch_bytes.restype = c_size_t
     lib.gsr_knn_mean_dist2.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.gsr_knn_mean_dist2.restype = c_int
+    lib.gsr_ssim_forward.argtypes = [c_int, c_int, c_int] + [c_void_p] * 5
+    lib.gsr_ssim_forward.restype = c_int
+    lib.gsr_ssim_backward.argtypes = [c_int, c_int, c_int] + [c_void_p] * 6
+    lib.gsr_ssim_backward.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

@@ -18,7 +18,8 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 * both rasterizer passes share one projection / depth order / tile binning (the drop-in package's geometry reuse).
 
 ``add_densification_stats`` (model method) / ``densification_stats`` (function) fuse method.py:1997-1998 and :1470-1477
-into one kernel.  Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
+into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``.
+Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
 ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features); anything else falls through to the original
 method, so ``enable`` is always safe.
 """
@@ -212,14 +213,36 @@ def compute_3D_filter(model, cameras) -> None:
         model.register_buffer("filter_3D", filter_3D[..., None])
 
 
-def enable(model, optimizer: bool = True):
+def _ssim_hook(original):
+    """A stand-in for method.py's module-level ``ssim`` (:644-673): ``fused_ssim.ssim`` where it supports the input,
+    ``original`` otherwise (CPU tensors, other dtypes or window sizes, a gradient wanted for img2, ...)."""
+    import fused_ssim
+
+    def ssim(img1, img2, window_size=11, size_average=True):
+        if fused_ssim.supported(img1, img2, window_size):
+            return fused_ssim.ssim(img1, img2, window_size, size_average)
+        return original(img1, img2, window_size, size_average)
+
+    ssim.__wrapped__ = original
+    return ssim
+
+
+def enable(model, optimizer: bool = True, ssim: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
-    class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place."""
+    class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
+
+    With ``ssim``, the module-level ``ssim`` of the model's method module (the photometric loss, method.py:1949, and
+    appearance optimisation, :1801) is rebound to ``fused_ssim.ssim`` for supported input.  That name is shared by every
+    model of the module; ``disable`` restores the original."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
         import fused_adam
         fused_adam.adopt(model.optimizer)
+    if ssim:
+        m = sys.modules[type(model).__module__]
+        if not hasattr(m.ssim, "__wrapped__"):
+            m.ssim = _ssim_hook(m.ssim)
     return model
 
 
@@ -228,4 +251,7 @@ def disable(model):
     model.__dict__.pop("compute_3D_filter", None)
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
+    m = sys.modules.get(type(model).__module__)
+    if m is not None and hasattr(getattr(m, "ssim", None), "__wrapped__"):
+        m.ssim = m.ssim.__wrapped__
     return model
