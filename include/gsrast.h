@@ -366,6 +366,22 @@ int gsr_ssim_forward(int B, int H, int W, const float* img1, const float* img2, 
 int gsr_ssim_backward(int B, int H, int W, const float* img1, const float* img2, const float* partials, const float* dL_dmap,
                       float* dL_dimg1, void* stream);
 
+/* -- Image-quality statistics of the uncertainty loss (optional entry points, forward only) -----------------------------
+ * `msssim(x, y, max_size, min_size)` and `ssim_down(x, y, max_size)` of wildgaussians/method.py:126-187.  img1, img2:
+ * [B,3,H,W] fp32, contiguous, on the device; out: [B,H,W].  (h, w) is the area-resize size the caller computed with
+ * the reference's own expression (F.interpolate(scale_factor=s, mode='area') gives int(H * s)); h == H && w == W means
+ * no resize.  The images are area-resized to (h, w), evaluated there, and the result bilinearly upsampled back to (H, W).
+ * msssim: level 0 contributes l*c*s, each 2x2-pooled level (while both sides exceed min_size) its c and s, upsampled to
+ * level 0 separately; the product is averaged over the channels.  ssim_down: the SSIM map of gsr_ssim_forward.
+ * scratch: device memory of gsr_*_scratch_bytes bytes (ssim_down needs none without a resize).  B <= 65535,
+ * min_size >= 1.  No host synchronisation.                                                                                */
+size_t gsr_msssim_scratch_bytes(int B, int h, int w, int min_size);   /* 0 for invalid sizes */
+int gsr_msssim_forward(int B, int H, int W, int h, int w, int min_size, const float* img1, const float* img2, float* out,
+                       void* scratch, void* stream);
+size_t gsr_ssim_down_scratch_bytes(int B, int h, int w);              /* 0 for invalid sizes */
+int gsr_ssim_down_forward(int B, int H, int W, int h, int w, const float* img1, const float* img2, float* out,
+                          void* scratch, void* stream);
+
 /* Optional per-stage device timing (cudaEvents on the caller's stream around each stage of the
  * next forward / backward calls).  The caller synchronises the stream, then reads the stage times of
  * the most recent calls in milliseconds (-1 for stages that did not run).  Not thread-safe.        */

@@ -13,8 +13,7 @@
 // Traffic: forward reads 24 B and writes 4 B (+ 36 B of factors) per pixel, backward reads 24 + 36 + 4 B and writes
 // 12 B per pixel; no atomics, so results are bitwise reproducible.
 //
-// Window: the reference's 1-D Gaussian (sigma 1.5, 11 taps) built in fp32 -- fp32(exp(.)) / fp32 sum -- applied
-// separably; its 2-D window is the fp32 outer product of the same vector.
+// Window, tile geometry and the separable blur: ssim_common.cuh.
 //
 // Backward, per channel, with window sums over pixels inside the image (the window is symmetric):
 //     mu_x = w*x,  E_xx = w*x^2,  E_xy = w*xy,  sigma_x^2 = E_xx - mu_x^2,  sigma_xy = E_xy - mu_x mu_y
@@ -25,52 +24,9 @@
 //     dS/dE_xy = 2 A1 / (B1 B2)
 //     dL/dx_p  = w*(g dS/dmu_x)_p + 2 x_p w*(g dS/dE_xx)_p + y_p w*(g dS/dE_xy)_p,   g = dL/dmap / 3
 // None of the factors divides by A1 or A2, so they stay finite where A2 <= 0.
-#include "common.cuh"
-
-#include <math.h>
+#include "ssim_common.cuh"
 
 namespace gsr {
-
-constexpr int SSIM_TW = 32;                       // output tile width (one warp per tile row)
-constexpr int SSIM_TH = 16;                       // output tile height
-constexpr int SSIM_R = 5;                         // window radius (window_size 11)
-constexpr int SSIM_K = 2 * SSIM_R + 1;
-constexpr int SSIM_RW = SSIM_TW + 2 * SSIM_R;     // staged region: tile plus halo
-constexpr int SSIM_RH = SSIM_TH + 2 * SSIM_R;
-constexpr int SSIM_THREADS = 256;
-constexpr int SSIM_PPT = SSIM_TW * SSIM_TH / SSIM_THREADS;   // output pixels per thread
-constexpr float SSIM_C1 = (float)(0.01 * 0.01);       // method.py:665-666, Python doubles rounded to fp32
-constexpr float SSIM_C2 = (float)(0.03 * 0.03);
-static_assert(SSIM_TW * SSIM_TH % SSIM_THREADS == 0, "whole pixels per thread");
-
-struct SsimWindow {
-    float w[SSIM_K];
-};
-
-// The reference's 1-D window (method.py:648-649): fp32(exp(-(x - 5)^2 / (2 sigma^2))), divided by the fp32 sum of those
-// taps.  The sum is accumulated in double and rounded once, which reproduces PyTorch's `gauss.sum()` here; a plain fp32
-// running sum lands one ulp away, and since sigma^2 = E[x^2] - mu^2 is sensitive to the window's total weight, that ulp
-// shows up as a systematic ~1e-6 offset of the SSIM mean.
-static SsimWindow ssim_window() {
-    SsimWindow g;
-    double sum = 0.0;
-    for (int x = 0; x < SSIM_K; ++x) {
-        g.w[x] = (float)exp(-(double)((x - SSIM_R) * (x - SSIM_R)) / (2.0 * 1.5 * 1.5));
-        sum += g.w[x];
-    }
-    const float fsum = (float)sum;
-    for (int x = 0; x < SSIM_K; ++x) g.w[x] = g.w[x] / fsum;
-    return g;
-}
-
-// Stage the tile's region of one channel plane into `dst`, zeros outside the image.
-__device__ __forceinline__ void ssim_stage(float (*dst)[SSIM_RW], const float* __restrict__ src, int H, int W, int x0, int y0) {
-    for (int i = threadIdx.x; i < SSIM_RH * SSIM_RW; i += SSIM_THREADS) {
-        const int r = i / SSIM_RW, q = i - r * SSIM_RW;
-        const int gy = y0 - SSIM_R + r, gx = x0 - SSIM_R + q;
-        dst[r][q] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? src[(size_t)gy * W + gx] : 0.f;
-    }
-}
 
 __global__ void __launch_bounds__(SSIM_THREADS) ssim_fwd_kernel(int H, int W, const float* __restrict__ img1,
                                                                 const float* __restrict__ img2, float* __restrict__ ssim_map,
@@ -89,37 +45,15 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_fwd_kernel(int H, int W, co
         ssim_stage(sx, img1 + plane, H, W, x0, y0);
         ssim_stage(sy, img2 + plane, H, W, x0, y0);
         __syncthreads();
-        // horizontal pass over every staged row: 5 moments per (row, output column)
-        for (int i = threadIdx.x; i < SSIM_RH * SSIM_TW; i += SSIM_THREADS) {
-            const int r = i / SSIM_TW, q = i - r * SSIM_TW;
-            float m0 = 0.f, m1 = 0.f, m2 = 0.f, m3 = 0.f, m4 = 0.f;
-#pragma unroll
-            for (int k = 0; k < SSIM_K; ++k) {
-                const float x = sx[r][q + k], y = sy[r][q + k], w = win.w[k];
-                m0 = fmaf(w, x, m0);
-                m1 = fmaf(w, y, m1);
-                m2 = fmaf(w, x * x, m2);
-                m3 = fmaf(w, y * y, m3);
-                m4 = fmaf(w, x * y, m4);
-            }
-            hb[0][r][q] = m0; hb[1][r][q] = m1; hb[2][r][q] = m2; hb[3][r][q] = m3; hb[4][r][q] = m4;
-        }
+        ssim_blur_rows(sx, sy, hb, win);
         __syncthreads();
         // vertical pass + the per-channel SSIM and its backward factors
 #pragma unroll
         for (int j = 0; j < SSIM_PPT; ++j) {
             const int i = threadIdx.x + j * SSIM_THREADS;
             const int r = i / SSIM_TW, q = i - r * SSIM_TW;
-            float mx = 0.f, my = 0.f, exx = 0.f, eyy = 0.f, exy = 0.f;
-#pragma unroll
-            for (int k = 0; k < SSIM_K; ++k) {
-                const float w = win.w[k];
-                mx = fmaf(w, hb[0][r + k][q], mx);
-                my = fmaf(w, hb[1][r + k][q], my);
-                exx = fmaf(w, hb[2][r + k][q], exx);
-                eyy = fmaf(w, hb[3][r + k][q], eyy);
-                exy = fmaf(w, hb[4][r + k][q], exy);
-            }
+            float mx, my, exx, eyy, exy;
+            ssim_blur_column(hb, r, q, win, mx, my, exx, eyy, exy);
             const float mxx = mx * mx, myy = my * my, mxy = mx * my;
             const float A1 = 2.f * mxy + SSIM_C1, A2 = 2.f * (exy - mxy) + SSIM_C2;
             const float B1 = mxx + myy + SSIM_C1, B2 = (exx - mxx) + (eyy - myy) + SSIM_C2;
@@ -210,10 +144,6 @@ static int ssim_check_sizes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) { set_error("bad sizes B=%d H=%d W=%d", B, H, W); return GSR_E_INVALID; }
     if (B > 65535 || (H + SSIM_TH - 1) / SSIM_TH > 65535) { set_error("image batch or height too large (B=%d H=%d)", B, H); return GSR_E_INVALID; }
     return 0;
-}
-
-static dim3 ssim_grid(int B, int H, int W) {
-    return dim3((W + SSIM_TW - 1) / SSIM_TW, (H + SSIM_TH - 1) / SSIM_TH, B);
 }
 
 }  // namespace gsr

@@ -131,6 +131,14 @@ def _load():
     lib.gsr_ssim_forward.restype = c_int
     lib.gsr_ssim_backward.argtypes = [c_int, c_int, c_int] + [c_void_p] * 6
     lib.gsr_ssim_backward.restype = c_int
+    lib.gsr_msssim_scratch_bytes.argtypes = [c_int] * 4
+    lib.gsr_msssim_scratch_bytes.restype = c_size_t
+    lib.gsr_msssim_forward.argtypes = [c_int] * 6 + [c_void_p] * 5
+    lib.gsr_msssim_forward.restype = c_int
+    lib.gsr_ssim_down_scratch_bytes.argtypes = [c_int] * 3
+    lib.gsr_ssim_down_scratch_bytes.restype = c_size_t
+    lib.gsr_ssim_down_forward.argtypes = [c_int] * 5 + [c_void_p] * 5
+    lib.gsr_ssim_down_forward.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

@@ -18,7 +18,8 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 * both rasterizer passes share one projection / depth order / tile binning (the drop-in package's geometry reuse).
 
 ``add_densification_stats`` (model method) / ``densification_stats`` (function) fuse method.py:1997-1998 and :1470-1477
-into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``.
+into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``, and
+``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187).
 Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
 ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features); anything else falls through to the original
 method, so ``enable`` is always safe.
@@ -227,13 +228,29 @@ def _ssim_hook(original):
     return ssim
 
 
-def enable(model, optimizer: bool = True, ssim: bool = False):
+def _stats_hook(original, fused, supported):
+    """A stand-in for method.py's module-level ``msssim`` (:171-187) or ``ssim_down`` (:126-135): the fused forward where
+    it supports the input, ``original`` otherwise (CPU tensors, other dtypes or shapes, a gradient wanted, ...)."""
+
+    def hook(*args, **kwargs):
+        if supported(*args, **kwargs):
+            return fused(*args, **kwargs)
+        return original(*args, **kwargs)
+
+    hook.__name__ = getattr(original, "__name__", fused.__name__)
+    hook.__wrapped__ = original
+    return hook
+
+
+def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
     With ``ssim``, the module-level ``ssim`` of the model's method module (the photometric loss, method.py:1949, and
-    appearance optimisation, :1801) is rebound to ``fused_ssim.ssim`` for supported input.  That name is shared by every
-    model of the module; ``disable`` restores the original."""
+    appearance optimisation, :1801) is rebound to ``fused_ssim.ssim`` for supported input.  With ``msssim``, its
+    ``msssim`` and ``ssim_down`` (the uncertainty loss, method.py:360, :368-369, :407) are rebound to ``fused_ssim.msssim``
+    and ``fused_ssim.ssim_down`` for supported input.  Those names are shared by every model of the module; ``disable``
+    restores the originals."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
@@ -243,6 +260,13 @@ def enable(model, optimizer: bool = True, ssim: bool = False):
         m = sys.modules[type(model).__module__]
         if not hasattr(m.ssim, "__wrapped__"):
             m.ssim = _ssim_hook(m.ssim)
+    if msssim:
+        import fused_ssim
+        m = sys.modules[type(model).__module__]
+        if not hasattr(m.msssim, "__wrapped__"):
+            m.msssim = _stats_hook(m.msssim, fused_ssim.msssim, fused_ssim.supported_msssim)
+        if not hasattr(m.ssim_down, "__wrapped__"):
+            m.ssim_down = _stats_hook(m.ssim_down, fused_ssim.ssim_down, fused_ssim.supported_ssim_down)
     return model
 
 
@@ -252,6 +276,8 @@ def disable(model):
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
     m = sys.modules.get(type(model).__module__)
-    if m is not None and hasattr(getattr(m, "ssim", None), "__wrapped__"):
-        m.ssim = m.ssim.__wrapped__
+    if m is not None:
+        for name in ("ssim", "msssim", "ssim_down"):
+            if hasattr(getattr(m, name, None), "__wrapped__"):
+                setattr(m, name, getattr(m, name).__wrapped__)
     return model
