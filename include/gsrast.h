@@ -382,6 +382,15 @@ size_t gsr_ssim_down_scratch_bytes(int B, int h, int w);              /* 0 for i
 int gsr_ssim_down_forward(int B, int H, int W, int h, int w, const float* img1, const float* img2, float* out,
                           void* scratch, void* stream);
 
+/* -- Attention of the DINOv2 backbone (optional entry points, forward only) ---------------------------------------------
+ * The core of `Attention.forward` (wildgaussians/dinov2.py:224-233) for 64-wide heads: softmax((q / 8) k^T) v per head.
+ * qkv: the `qkv` Linear's output [B][N][3][H][64] fp32, contiguous, 16-byte aligned, on the device; out: [B][N][H * 64]
+ * fp32 (heads concatenated, the input of `proj`).  Exact softmax with 3xTF32 tensor-core products.  scratch: device
+ * memory of gsr_attention_scratch_bytes bytes (B * H * ceil(N / 64) * 80 KB).  B <= 65535, H <= 65535, N >= 1.
+ * Two launches, no atomics, no host synchronisation.                                                                     */
+size_t gsr_attention_scratch_bytes(int B, int N, int H);            /* 0 for invalid sizes */
+int gsr_attention_forward(int B, int N, int H, const float* qkv, float* out, void* scratch, void* stream);
+
 /* Optional per-stage device timing (cudaEvents on the caller's stream around each stage of the
  * next forward / backward calls).  The caller synchronises the stream, then reads the stage times of
  * the most recent calls in milliseconds (-1 for stages that did not run).  Not thread-safe.        */

@@ -1,5 +1,5 @@
 // wgmma.cuh -- thin inline-PTX layer over Hopper's warpgroup tensor-core instructions (wgmma), mbarriers and 1-D bulk
-// asynchronous copies, as used by appearance.cu.  sm_90a only.
+// asynchronous copies, as used by appearance.cu and attention.cu.  sm_90a only.
 //
 // Operand storage convention ("rows16"): a bf16 matrix X[ROWS][COLS] lives in shared memory as
 //     byte address(row, col) = (col / 8) * (ROWS * 16) + row * 16 + (col % 8) * 2
@@ -66,6 +66,25 @@ __device__ __forceinline__ void mma_n144(float (&d)[72], uint64_t da, uint64_t d
                  : "l"(da), "l"(db), "r"((uint32_t)accumulate), "n"(TA), "n"(TB));
 }
 
+// ---- wgmma: D[64 x 64] (+)= A[64 x 8] B[8 x 64], tf32 operands, fp32 accumulators ----------------------------------
+// TF32 operands in shared memory are K-major only (no transpose immediates).  In rows16 storage a 16-byte unit holds 4
+// tf32 columns, so a K-major operand X[ROWS][COLS] lives at (col / 4) * (ROWS * 16) + row * 16 + (col % 4) * 4 with
+// SBO = 128 B and LBO = ROWS * 16 B; one K = 8 step advances the start address by 2 * ROWS * 16 B.
+// A from registers: warp w of the warpgroup, lane l holds rows r = 16 w + l / 4 and r + 8, columns c = l % 4 and c + 4:
+//     a[0] = A(r, c), a[1] = A(r + 8, c), a[2] = A(r, c + 4), a[3] = A(r + 8, c + 4)   (tf32 bit patterns)
+__device__ __forceinline__ void mma_tf32_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, bool accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"((uint32_t)accumulate));
+}
+// the same with A K-major in shared memory
+__device__ __forceinline__ void mma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, bool accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"((uint32_t)accumulate));
+}
 
 __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void commit_group() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -84,6 +103,9 @@ __device__ __forceinline__ void warpgroup_sync(int w) { asm volatile("bar.sync %
 // ---- mbarrier ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -113,6 +135,17 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);      // .x = lo (low 16 bits)
     return *reinterpret_cast<const uint32_t*>(&v);
+}
+// x rounded to the nearest tf32 (10 explicit mantissa bits; the low 13 bits of the result are zero)
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+// 3xTF32 split: x = hi + lo + O(2^-22 |x|), both parts tf32
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+    hi = to_tf32(x);
+    lo = to_tf32(x - __uint_as_float(hi));
 }
 
 }  // namespace wg

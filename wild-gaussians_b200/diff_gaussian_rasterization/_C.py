@@ -139,6 +139,10 @@ def _load():
     lib.gsr_ssim_down_scratch_bytes.restype = c_size_t
     lib.gsr_ssim_down_forward.argtypes = [c_int] * 5 + [c_void_p] * 5
     lib.gsr_ssim_down_forward.restype = c_int
+    lib.gsr_attention_scratch_bytes.argtypes = [c_int] * 3
+    lib.gsr_attention_scratch_bytes.restype = c_size_t
+    lib.gsr_attention_forward.argtypes = [c_int] * 3 + [c_void_p] * 4
+    lib.gsr_attention_forward.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

@@ -18,8 +18,10 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 * both rasterizer passes share one projection / depth order / tile binning (the drop-in package's geometry reuse).
 
 ``add_densification_stats`` (model method) / ``densification_stats`` (function) fuse method.py:1997-1998 and :1470-1477
-into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``, and
-``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187).
+into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``,
+``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187), and
+``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
+after the last block asked for, fused attention).
 Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
 ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features); anything else falls through to the original
 method, so ``enable`` is always safe.
@@ -242,7 +244,16 @@ def _stats_hook(original, fused, supported):
     return hook
 
 
-def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False):
+def dino_get_intermediate_layers(self, x, n=1, reshape=False, return_class_token=False, norm=True):
+    """Drop-in for ``DinoVisionTransformer.get_intermediate_layers`` (dinov2.py:789-813): ``fused_dino`` where it supports
+    the input, the class's own method otherwise (CPU tensors, other dtypes, a gradient wanted, other head sizes, ...)."""
+    import fused_dino
+    if fused_dino.supported(self, x, n):
+        return fused_dino.get_intermediate_layers(self, x, n, reshape, return_class_token, norm)
+    return type(self).get_intermediate_layers(self, x, n, reshape, return_class_token, norm)
+
+
+def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -250,7 +261,8 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     appearance optimisation, :1801) is rebound to ``fused_ssim.ssim`` for supported input.  With ``msssim``, its
     ``msssim`` and ``ssim_down`` (the uncertainty loss, method.py:360, :368-369, :407) are rebound to ``fused_ssim.msssim``
     and ``fused_ssim.ssim_down`` for supported input.  Those names are shared by every model of the module; ``disable``
-    restores the originals."""
+    restores the originals.  With ``dino``, ``model.uncertainty_model.backbone.get_intermediate_layers`` (every DINOv2
+    call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
@@ -267,12 +279,22 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
             m.msssim = _stats_hook(m.msssim, fused_ssim.msssim, fused_ssim.supported_msssim)
         if not hasattr(m.ssim_down, "__wrapped__"):
             m.ssim_down = _stats_hook(m.ssim_down, fused_ssim.ssim_down, fused_ssim.supported_ssim_down)
+    backbone = _dino_backbone(model)
+    if dino and backbone is not None and "get_intermediate_layers" not in backbone.__dict__:
+        backbone.get_intermediate_layers = types.MethodType(dino_get_intermediate_layers, backbone)
     return model
+
+
+def _dino_backbone(model):
+    return getattr(getattr(model, "uncertainty_model", None), "backbone", None)
 
 
 def disable(model):
     model.__dict__.pop("_render_internal", None)
     model.__dict__.pop("compute_3D_filter", None)
+    backbone = _dino_backbone(model)
+    if backbone is not None:
+        backbone.__dict__.pop("get_intermediate_layers", None)
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
     m = sys.modules.get(type(model).__module__)
