@@ -228,6 +228,13 @@ int    gsr_backward_finalize_pull(const GsrBackwardArgs* args, const void* const
                                   const void* const* peer_touched, int n_peers, int self, void* clear_accum,
                                   unsigned char* clear_touched, void* stream);
 
+/* Colour gradient alone: dL_dcolor [P,3] = sum over the pixels of T alpha dL_dpix, the colour part of gsr_backward,
+ * for callers that optimise nothing but the colours (test-time appearance optimisation).  Reads P, M, R, W, H,
+ * subpixel_offset, geom_buffer, binning_buffer, img_buffer (that of the forward or of gsr_forward_recolor), dL_dpix,
+ * tile_y0 / tile_y1 and debug; every other field is ignored.  dL_dcolor is written completely (zero for Gaussians no
+ * pixel blends).                                                                                                        */
+int gsr_backward_colors(const GsrBackwardArgs* args, void* stream);
+
 /* -- markVisible (rasterizer_impl.cu:54-66,141-153): present[i] = (view*p).z > 0.2 ------- */
 int gsr_mark_visible(int P, const float* means3D, const float* viewmatrix,
                      const float* projmatrix, uint8_t* present, void* stream);
@@ -292,6 +299,12 @@ int gsr_appearance_colors_backward(const GsrAppearanceArgs* args, void* stream);
 int gsr_appearance_unpack_grads(const float* grad_pack, const float* W1, const float* appearance_embedding, float* dW1,
                                 float* db1, float* dW2, float* db2, float* dW3, float* db3,
                                 float* dappearance_embedding, void* stream);
+/* Gradient of the image embedding alone (test-time appearance optimisation, where nothing else is trained): recomputes
+ * the MLP like gsr_appearance_colors_backward and writes sum over the P rows of dL/d(layer-1 pre-activation) into the
+ * db1 slot of `grad_pack` (the rest of the image is zeroed); gsr_appearance_unpack_grads then gives d(image embedding)
+ * (and db1; its other outputs are zero).  Reads features_dc / features_rest / embeddings / means3D / campos /
+ * packed_weights / dL_dcolors_toned; every other pointer of `args` is ignored.  P = 0 is valid (a zero gradient).     */
+int gsr_appearance_embedding_backward(const GsrAppearanceArgs* args, void* stream);
 
 /* -- parameter activations + 3D filter (SURVEY.md 8f-2; optional entry points) --------------------------------------------
  * GaussianModel.get_gaussians (wildgaussians/method.py:1060-1086) in one kernel per direction: rotations = normalize(raw),

@@ -564,6 +564,32 @@ int gsr_backward(const GsrBackwardArgs* a, void* stream) {
     return gsr_backward_finalize(a, stream);
 }
 
+int gsr_backward_colors(const GsrBackwardArgs* a, void* stream) {
+    if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
+    if (a->P < 0 || a->M < 0 || a->W <= 0 || a->H <= 0 || a->R < 0) { set_error("bad sizes"); return GSR_E_INVALID; }
+    if (a->P == 0) return 0;
+    if (!a->geom_buffer || !a->img_buffer || !a->subpixel_offset || !a->dL_dpix || !a->dL_dcolor ||
+        (a->R > 0 && !a->binning_buffer)) {
+        set_error("a required pointer is NULL");
+        return GSR_E_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    GSR_CUDA(cudaMemsetAsync(a->dL_dcolor, 0, (size_t)a->P * 3 * sizeof(float), s));
+    if (a->R == 0) return 0;
+    GeomState g;
+    ImgState im;
+    BinState b;
+    carve_geom((char*)a->geom_buffer, a->P, a->M, &g);
+    carve_img((char*)a->img_buffer, a->W, a->H, &im);
+    carve_bin((char*)a->binning_buffer, (size_t)a->R, &b);
+    int ty0, ty1;
+    shard_rows(a->H, a->tile_y0, a->tile_y1, &ty0, &ty1);
+    int rc = launch_render_color_grad(*a, g, b, im, ty0, ty1, s);
+    if (rc) return rc;
+    GSR_STAGE(s, a->debug != 0, "render_color_grad_kernel");
+    return 0;
+}
+
 int gsr_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present,
                      void* stream) {
     (void)projmatrix;

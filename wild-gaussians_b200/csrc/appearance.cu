@@ -627,6 +627,212 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __
     }
 }
 
+// =====================================================================================================================
+// embedding-only backward (test-time appearance optimisation)
+// =====================================================================================================================
+// When only the image embedding is optimised, its gradient is W1[:, 27:59]^T . sum_rows dZ1 (the embedding is folded
+// into the layer-1 bias), and the unpack kernel forms that product from the db1 slot of the gradient image.  This kernel
+// therefore recomputes the three layers per tile as appearance_bwd_kernel does, runs dO -> dZ2 -> dZ1 and accumulates
+// only sum_rows dZ1: no weight-gradient GEMM, no dX, no per-Gaussian input gradient.  The ReLU masks of H1 and H2 stay
+// in registers (the dH accumulators have the layout of the forward accumulators), so one activation image serves all
+// layers, dO reuses the layer-3 output rows and the per-warp column sums reuse the SH staging area: the shared memory
+// is the forward kernel's and two CTAs fit an SM.
+
+// relu_epilogue, also returning which of this thread's 64 accumulator entries are positive after the bf16 rounding
+// (bit i of pos[i / 32] for d[i]), the mask relu_bwd_epilogue reads back from the activation image
+__device__ __forceinline__ void relu_epilogue_mask(const float (&d)[64], uint8_t* hbuf, Frag f, uint32_t (&pos)[2]) {
+    pos[0] = pos[1] = 0u;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const uint32_t a = pack_bf16(fmaxf(d[4 * j], 0.f), fmaxf(d[4 * j + 1], 0.f));
+        const uint32_t b = pack_bf16(fmaxf(d[4 * j + 2], 0.f), fmaxf(d[4 * j + 3], 0.f));
+        st_pair(hbuf, j, f.r0, f.c, a);
+        st_pair(hbuf, j, f.r0 + 8, f.c, b);
+        const uint32_t m = ((a & 0x7FFFu) ? 1u : 0u) | ((a & 0x7FFF0000u) ? 2u : 0u) | ((b & 0x7FFFu) ? 4u : 0u) |
+                           ((b & 0x7FFF0000u) ? 8u : 0u);
+        pos[j >> 3] |= m << (4 * (j & 7));
+    }
+}
+__device__ __forceinline__ float masked_bf16(const uint32_t (&pos)[2], int i, float v) {
+    return ((pos[i >> 5] >> (i & 31)) & 1u) ? __bfloat162float(__float2bfloat16(v)) : 0.f;
+}
+
+// the RowIn that build_x_row returns for a valid row (same expressions, so the same bits)
+__device__ __forceinline__ void row_in(const ApParams& p, int row, RowIn& in) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) in.dc[c] = p.dc[(size_t)row * 3 + c];
+    const float vx = p.means[(size_t)row * 3 + 0] - p.campos[0], vy = p.means[(size_t)row * 3 + 1] - p.campos[1],
+                vz = p.means[(size_t)row * 3 + 2] - p.campos[2];
+    const float nrm = fmaxf(sqrtf(vx * vx + vy * vy + vz * vz), 1e-12f);
+    in.inv_norm = 1.0f / nrm;
+    in.dir = {vx * in.inv_norm, vy * in.inv_norm, vz * in.inv_norm};
+}
+
+// dL/d(o) of the toned colour of one row (o = the six MLP outputs before the x 0.01): the colour-stage backward of
+// appearance_bwd_kernel restricted to the toned path
+__device__ __forceinline__ void toned_dout(int deg, const RowIn& in, const float* o, const float* fr, const float* dL_toned,
+                                           float (&dOut)[AP_NOUT]) {
+    float b[16];
+    sh_basis(deg, in.dir.x, in.dir.y, in.dir.z, b);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float mul = 0.01f * o[3 + c], off = 0.01f * o[c] / SH_C0;
+        const float f0 = fminf(in.dc[c], 1.0f);
+        const float t0p = fmaf(f0, mul, off);
+        float s = b[0] * fminf(t0p, 1.0f);
+#pragma unroll
+        for (int k = 1; k < 16; ++k) s = fmaf(b[k], fminf(fminf(fr[3 * (k - 1) + c], 1.0f) * mul, 1.0f), s);
+        const float dLt = (s + 0.5f >= 0.f) ? dL_toned[c] : 0.f;
+        const float dt0 = (t0p <= 1.0f) ? b[0] * dLt : 0.f;
+        float dmul = dt0 * f0;
+        dOut[c] = 0.01f * dt0 / SH_C0;
+#pragma unroll
+        for (int k = 1; k < 16; ++k) {
+            const float fv = fminf(fr[3 * (k - 1) + c], 1.0f);
+            const float dt = (fv * mul <= 1.0f) ? b[k] * dLt : 0.f;
+            dmul = fmaf(dt, fv, dmul);
+        }
+        dOut[3 + c] = 0.01f * dmul;
+    }
+}
+
+__global__ void __launch_bounds__(FWD_THREADS, 2) appearance_emb_bwd_kernel(const __grid_constant__ ApParams p) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint8_t* s_blob = smem;
+    uint8_t* s_act = smem + BLOB_BYTES;
+    float* s_rest = reinterpret_cast<float*>(smem + BLOB_BYTES + ACT_BYTES);
+    float* s_out = reinterpret_cast<float*>(smem + BLOB_BYTES + ACT_BYTES + REST_BYTES);
+    uint8_t* s_do = reinterpret_cast<uint8_t*>(s_out);        // dO image (2 chunks) over the consumed layer-3 output rows
+    float* s_colsum = s_rest;                                 // [8 warps][128] dZ1 column sums over the consumed SH rows
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BLOB_BYTES + ACT_BYTES + REST_BYTES + OUT_BYTES);
+    const int tid = threadIdx.x, t = tid & (AP_TILE - 1), w = tid >> 7, lane = tid & 31, warp = tid >> 5;
+    const bool h0 = w == 0;
+    const Frag f = frag_of(tid);
+
+    if (tid == 0) {
+        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
+        mbar_init_fence();
+    }
+    if (h0) write_const_chunks(s_act, t);
+    fence_async_smem();
+    __syncthreads();
+    if (tid == 0) {
+        mbar_expect_tx(&bars[1], BLOB_BYTES);
+        bulk_g2s(s_blob, p.blob, BLOB_BYTES, &bars[1]);
+    }
+    const uint8_t* w1p = s_blob;
+    const uint8_t* w2p = s_blob + W1P_BYTES;
+    const uint8_t* w3p = w2p + W2P_BYTES;
+    float acc[64], acc3[8];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc3[i] = 0.f;
+    float colsum = 0.f;                                       // thread n < 128: sum of dZ1[:, n] over this CTA's tiles
+    uint32_t ph_ld = 0;
+    bool dead = false;
+    if (!mbar_wait(&bars[1], 0)) AP_FAIL();
+
+    for (int tile = blockIdx.x; tile < p.num_tiles && !dead; tile += gridDim.x) {
+        const int row0 = tile * AP_TILE, row = row0 + t;
+        const int rows = min(AP_TILE, p.P - row0);
+        const bool valid = h0 && t < rows;
+        const bool bulk = rows == AP_TILE;
+        if (bulk) {
+            if (tid == 0) {
+                mbar_expect_tx(&bars[0], REST_BYTES);
+                bulk_g2s(s_rest, p.rest + (size_t)row0 * AP_NREST, REST_BYTES, &bars[0]);
+            }
+        } else {
+            for (int i = tid; i < rows * AP_NREST; i += FWD_THREADS) s_rest[i] = p.rest[(size_t)row0 * AP_NREST + i];
+        }
+        {   // the row input is read again for the colour stage rather than held across the GEMMs (register budget)
+            RowIn in;
+            if (h0) build_x_row(p, row, valid, t, s_act, in);
+        }
+        fence_async_smem();
+        __syncthreads();
+        // ---- forward recompute (a warpgroup reads and overwrites only its own 64 rows) -----------------------------------
+        uint32_t pos1[2], pos2[2];
+        gemm_n128<AP_K1 / 16>(acc, s_act, w1p, w);
+        relu_epilogue_mask(acc, s_act, f, pos1);
+        fence_async_smem();
+        warpgroup_sync(w);
+        gemm_n128<AP_K2 / 16>(acc, s_act, w2p, w);
+        relu_epilogue_mask(acc, s_act, f, pos2);
+        fence_async_smem();
+        warpgroup_sync(w);
+        gemm_n16(acc3, s_act, w3p, w);
+        store_out(acc3, s_out, f);
+        __syncthreads();
+        if (bulk) {
+            if (!mbar_wait(&bars[0], ph_ld)) AP_FAIL();
+            ph_ld ^= 1u;
+        }
+        // ---- colour stage: dL/d(toned) -> dO ------------------------------------------------------------------------
+        float dOut[AP_NOUT] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (valid) {
+            RowIn in;
+            row_in(p, row, in);
+            toned_dout(p.deg, in, s_out + t * 8, s_rest + t * AP_NREST, p.dL_toned + (size_t)row * 3, dOut);
+        }
+        __syncthreads();          // every row of s_out and s_rest has been read: both are rewritten below
+        if (h0) {
+            st_chunk(s_do, 0, t, make_uint4(pack_bf16(dOut[0], dOut[1]), pack_bf16(dOut[2], dOut[3]), pack_bf16(dOut[4], dOut[5]), 0u));
+            st_chunk(s_do, 1, t, make_uint4(0u, 0u, 0u, 0u));
+        }
+        fence_async_smem();
+        __syncthreads();
+        // ---- dH2 = dO . W3 -> dZ2 (bf16, over H2 in the activation image) -------------------------------------------------
+        // (the GEMM does not accumulate: clearing acc ends the previous GEMM's live range before the colour stage)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        fence_regs(acc);
+        fence();
+        mma_n128<0, 1>(acc, desc_k(s_do + w * 1024, 0, AP_TILE), desc_mn(w3p, 0, AP_N3), false);
+        commit_group();
+        wait_all();
+        fence_regs(acc);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            st_pair(s_act, j, f.r0, f.c, pack_bf16(masked_bf16(pos2, 4 * j, acc[4 * j]), masked_bf16(pos2, 4 * j + 1, acc[4 * j + 1])));
+            st_pair(s_act, j, f.r0 + 8, f.c,
+                    pack_bf16(masked_bf16(pos2, 4 * j + 2, acc[4 * j + 2]), masked_bf16(pos2, 4 * j + 3, acc[4 * j + 3])));
+        }
+        fence_async_smem();
+        warpgroup_sync(w);
+        // ---- dH1 = dZ2 . W2 -> dZ1 (bf16, as the weight-gradient GEMM of appearance_bwd_kernel reads it) -------------------
+        fence_regs(acc);
+        fence();
+#pragma unroll
+        for (int k = 0; k < AP_H / 16; ++k) mma_n128<0, 1>(acc, desc_k(s_act + w * 1024, k, AP_TILE), desc_mn(w2p, k, AP_H), k > 0);
+        commit_group();
+        wait_all();
+        fence_regs(acc);
+        // column sums of dZ1: this thread's two rows, then the 8 row groups of the warp (lanes differing in bits 2..4)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            float s0 = masked_bf16(pos1, 4 * j, acc[4 * j]) + masked_bf16(pos1, 4 * j + 2, acc[4 * j + 2]);
+            float s1 = masked_bf16(pos1, 4 * j + 1, acc[4 * j + 1]) + masked_bf16(pos1, 4 * j + 3, acc[4 * j + 3]);
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+                s0 += __shfl_xor_sync(0xFFFFFFFFu, s0, o);
+                s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, o);
+            }
+            if (lane < 4) *reinterpret_cast<float2*>(s_colsum + warp * AP_H + 8 * j + 2 * f.c) = make_float2(s0, s1);
+        }
+        __syncthreads();
+        if (tid < AP_H) {
+#pragma unroll
+            for (int k = 0; k < FWD_THREADS / 32; ++k) colsum += s_colsum[k * AP_H + tid];
+        }
+        fence_async_smem();       // generic accesses of s_rest / s_act are ordered before the next tile's bulk copy into them
+        __syncthreads();
+    }
+    // db1 slot of the gradient image: dW1p[n][AP_ONE1] = sum over the Gaussians of dZ1[:, n] (X[:, AP_ONE1] = 1)
+    if (tid < AP_H && !dead && blockIdx.x < p.num_tiles) atomicAdd(p.g_pack + GW1P + (size_t)tid * AP_K1 + AP_ONE1, colsum);
+}
+
 // ---- host side ----------------------------------------------------------------------------------------------------
 static int ap_num_sms() {
     static int n = 0;
@@ -714,6 +920,34 @@ int gsr_appearance_colors_backward(const GsrAppearanceArgs* a, void* stream) {
     GSR_CUDA(cudaFuncSetAttribute(appearance_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM));
     const int grid = min(p.num_tiles, ap_num_sms());          // persistent: one CTA per SM (187 KB of shared memory)
     appearance_bwd_kernel<<<grid, BWD_THREADS, BWD_SMEM, s>>>(p);
+    count_launches(1);
+    GSR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int gsr_appearance_embedding_backward(const GsrAppearanceArgs* a, void* stream) {
+    if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
+    if (a->P < 0 || a->sh_degree < 0 || a->sh_degree > 3) { set_error("bad P / sh_degree"); return GSR_E_INVALID; }
+    if (!a->grad_pack) { set_error("grad_pack is NULL"); return GSR_E_INVALID; }
+    if (a->P > 0) {
+        if (!a->features_dc || !a->features_rest || !a->embeddings || !a->means3D || !a->campos || !a->packed_weights ||
+            !a->dL_dcolors_toned) {
+            set_error("a required pointer is NULL");
+            return GSR_E_INVALID;
+        }
+        if ((reinterpret_cast<uintptr_t>(a->features_rest) | reinterpret_cast<uintptr_t>(a->embeddings) |
+             reinterpret_cast<uintptr_t>(a->packed_weights)) & 15u) {
+            set_error("features_rest / embeddings / packed_weights must be 16-byte aligned");
+            return GSR_E_INVALID;
+        }
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    GSR_CUDA(cudaMemsetAsync(a->grad_pack, 0, GPACK_FLOATS * sizeof(float), s));
+    if (a->P == 0) return 0;
+    const ApParams p = ap_params(a);
+    GSR_CUDA(cudaFuncSetAttribute(appearance_emb_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM));
+    const int grid = min(p.num_tiles, 2 * ap_num_sms());      // persistent: two resident CTAs per SM, as the forward
+    appearance_emb_bwd_kernel<<<grid, FWD_THREADS, FWD_SMEM, s>>>(p);
     count_launches(1);
     GSR_CUDA(cudaGetLastError());
     return 0;

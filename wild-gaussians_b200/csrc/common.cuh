@@ -161,6 +161,9 @@ int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R, size_t N
 
 int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, int ty0, int ty1, cudaStream_t s);
+// colour-only backward composite (render_fwd.cu): adds sum T alpha dL/dpixel into a.dL_dcolor
+int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im, int ty0,
+                             int ty1, cudaStream_t s);
 
 struct BwdAccum { float4 a, b, c; };  // per-Gaussian packed partial gradients (48 B)
 // a = {dmean2D.x, dmean2D.y, |dmean2D|, dconic.x}  b = {dconic.y, dconic.w, dopacity, dcolor.r}

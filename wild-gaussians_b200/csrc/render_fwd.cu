@@ -415,6 +415,177 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
     }
 }
 
+// ---- colour-only backward: dL/dcolour = sum over pixels of T alpha dL/dpixel -------------------------------------------
+// When only the colours change (test-time appearance optimisation), the composite's gradient needs no conic, opacity or
+// mean terms, and the weight of a Gaussian at a pixel is the T alpha of the forward walk.  This kernel repeats the
+// packed forward's front-to-back walk with the same pair arithmetic, so T and alpha are the forward's bits, and
+// replaces the colour accumulation by the accumulation of T alpha dL/dpixel per Gaussian.  A pixel blends position i
+// iff i < n_contrib and the power / alpha tests pass (the position where a pixel saturates is never below n_contrib),
+// so the walk needs no saturation test; below MASK_K a warp walks exactly the positions the forward's blend mask marks
+// for its 8x8 block, above it the footprint culls as in the forward.  The three sums are reduced over the warp before
+// the global atomics.
+struct ColorGradParams {
+    int W, H, grid_x, ty0;
+    const uint2* ranges;
+    const uint32_t* point_list;
+    const float2* subpixel_offset;
+    const float4* rec;
+    const uint32_t* n_contrib;
+    const uint32_t* blend_mask;
+    const float* dL_dpix;      // [3,H,W]
+    float* dL_dcolor;          // [P,3], zeroed before the launch
+};
+
+// sum of (v0, v1, v2) over the warp in 6 shuffles (a 4-value butterfly with one padding slot); lane l ends up holding the
+// warp total of component 2 * bit4(l) + bit3(l) (3: padding)
+__device__ __forceinline__ float butterfly3(float v0, float v1, float v2, int lane) {
+    const bool h16 = lane & 16, h8 = lane & 8;
+    const float w0 = (h16 ? v2 : v0) + __shfl_xor_sync(0xFFFFFFFFu, h16 ? v0 : v2, 16);
+    const float w1 = (h16 ? 0.f : v1) + __shfl_xor_sync(0xFFFFFFFFu, h16 ? v1 : 0.f, 16);
+    float x = (h8 ? w1 : w0) + __shfl_xor_sync(0xFFFFFFFFu, h8 ? w0 : w1, 8);
+    x += __shfl_xor_sync(0xFFFFFFFFu, x, 4);
+    x += __shfl_xor_sync(0xFFFFFFFFu, x, 2);
+    x += __shfl_xor_sync(0xFFFFFFFFu, x, 1);
+    return x;
+}
+
+__global__ void __launch_bounds__(128) render_color_grad_kernel(const __grid_constant__ ColorGradParams p) {
+    using PM = PixelMap<2>;
+    constexpr int WARPS = PM::WARPS;
+    constexpr int PB = 128;               // instances per round (one per thread)
+    constexpr int NW = PB / 32;           // blend-mask words per round (rounds start at multiples of 32 positions)
+    __shared__ __align__(16) float4 s_xy[PB];    // {x, x, y, y}
+    __shared__ __align__(16) float4 s_ac[PB];    // {conic.x, conic.x, conic.z, conic.z}
+    __shared__ __align__(16) float4 s_bo[PB];    // {-conic.y, -conic.y, opacity, opacity}
+    __shared__ __align__(16) float4 s_geo[PB];   // {x, y, hx, hy} for the footprint culling
+    __shared__ uint32_t s_id[PB];
+    __shared__ uint32_t s_max[WARPS];
+    __shared__ uint32_t s_mask[WARPS][NW];
+    static_assert(WARPS == MASK_BLOCKS, "one warp per 8x8 blend-mask block");
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
+    const int tile = tile_y * p.grid_x + tile_x;
+    const size_t plane = (size_t)p.H * p.W;
+
+    float2 npx, npy, dL0, dL1, dL2;
+    uint32_t last0 = 0, last1 = 0;
+    float bx0 = 3.0e38f, bx1 = -3.0e38f, by0 = 3.0e38f, by1 = -3.0e38f;
+    {
+        float px[2], py[2], d0[2] = {0.f, 0.f}, d1[2] = {0.f, 0.f}, d2[2] = {0.f, 0.f};
+        uint32_t last[2] = {0u, 0u};
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            int lx, ly;
+            PM::pixel(tid, k, lx, ly);
+            const unsigned ux = tile_x * TILE + lx, uy = tile_y * TILE + ly;
+            const unsigned pix_id = p.W * uy + ux;
+            px[k] = (float)ux; py[k] = (float)uy;
+            if (ux < (unsigned)p.W && uy < (unsigned)p.H) {
+                const float2 so = p.subpixel_offset[pix_id];
+                px[k] += so.x; py[k] += so.y;
+                last[k] = p.n_contrib[pix_id];
+                d0[k] = p.dL_dpix[pix_id]; d1[k] = p.dL_dpix[plane + pix_id]; d2[k] = p.dL_dpix[2 * plane + pix_id];
+                bx0 = fminf(bx0, px[k]); bx1 = fmaxf(bx1, px[k]);
+                by0 = fminf(by0, py[k]); by1 = fmaxf(by1, py[k]);
+            }
+        }
+        npx = make_float2(-px[0], -px[1]); npy = make_float2(-py[0], -py[1]);
+        dL0 = make_float2(d0[0], d0[1]); dL1 = make_float2(d1[0], d1[1]); dL2 = make_float2(d2[0], d2[1]);
+        last0 = last[0]; last1 = last[1];
+    }
+    const WarpBox box = warp_box_reduce(bx0, bx1, by0, by1);
+    const uint2 range = p.ranges[tile];
+    const uint32_t warp_last = __reduce_max_sync(0xFFFFFFFFu, max(last0, last1));
+    if (lane == 0) s_max[warp] = warp_last;
+    __syncthreads();
+    uint32_t tile_last = 0;
+#pragma unroll
+    for (int k = 0; k < WARPS; ++k) tile_last = max(tile_last, s_max[k]);
+    const int total = (int)min(tile_last, range.y - range.x);   // nothing behind the tile's last contributor blends
+    const int rounds = (total + PB - 1) / PB;
+    const int comp = 2 * ((lane >> 4) & 1) + ((lane >> 3) & 1);   // component butterfly3 leaves in this lane
+    const bool owner = (lane & 7) == 0 && comp < 3;
+
+    float2 T = make_float2(1.f, 1.f);
+    const float2 mhalf = make_float2(-0.5f, -0.5f), one = make_float2(1.f, 1.f);
+    for (int r = 0; r < rounds; ++r) {
+        const int n = min(PB, total - r * PB);
+        __syncthreads();   // the previous round's staging is consumed
+        if (tid < n) {
+            const uint32_t id = p.point_list[range.x + r * PB + tid];
+            const float4* src = p.rec + 2 * (size_t)id;
+            const float4 g = src[0], c = src[1];
+            s_id[tid] = id;
+            s_geo[tid] = g;
+            s_xy[tid] = make_float4(g.x, g.x, g.y, g.y);
+            s_ac[tid] = make_float4(c.x, c.x, c.z, c.z);
+            s_bo[tid] = make_float4(-c.y, -c.y, c.w, c.w);
+        }
+        if (tid < WARPS * NW) {            // words at or above the block's largest n_contrib may be stale: read as 0
+            const int k = tid / NW, word = r * NW + tid % NW;
+            uint32_t m = 0;
+            if (word < MASK_WORDS && 32 * word < (int)s_max[k]) m = p.blend_mask[((size_t)tile * MASK_BLOCKS + k) * MASK_WORDS + word];
+            s_mask[k][tid % NW] = m;
+        }
+        __syncthreads();
+
+#pragma unroll 1
+        for (int w = 0; w < PB / 32; ++w) {
+            const int jl = w * 32 + lane;
+            const uint32_t pos = (uint32_t)(r * PB + jl);
+            bool rel = false;
+            if (jl < n && pos < warp_last) {
+                if (pos < (uint32_t)MASK_K) {
+                    rel = (s_mask[warp][w] >> lane) & 1u;
+                } else {
+                    const float4 g = s_geo[jl], bo = s_bo[jl], ac = s_ac[jl];
+                    rel = box_may_touch(g, box) && ellipse_may_touch(g.x, g.y, ac.x, -bo.x, ac.z, bo.z, box);
+                }
+            }
+            unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
+            while (mm) {
+                const int j = w * 32 + __ffs(mm) - 1;
+                mm &= mm - 1;
+                const uint32_t jpos = (uint32_t)(r * PB + j);
+                const float4 xy = s_xy[j], ac = s_ac[j], bo = s_bo[j];
+                // the packed forward's expressions (render_fwd_packed_kernel), so that T and alpha are its bits
+                const float2 dx = add2(make_float2(xy.x, xy.y), npx), dy = add2(make_float2(xy.z, xy.w), npy);
+                const float2 t1 = mul2(make_float2(ac.x, ac.y), dx);
+                const float2 t3 = mul2(dy, mul2(make_float2(ac.z, ac.w), dy));
+                const float2 un = mul2(dy, mul2(make_float2(bo.x, bo.y), dx));
+                const float2 power = fma2(fma2(dx, t1, t3), mhalf, un);
+                const float2 oG = mul2(make_float2(bo.z, bo.w), make_float2(expf(power.x), expf(power.y)));
+                const float a0 = min(0.99f, oG.x), a1 = min(0.99f, oG.y);
+                const float2 test_T = mul2(T, add2(one, make_float2(-a0, -a1)));
+                const bool upd0 = jpos < last0 && !(power.x > 0.0f) && !(a0 < 1.0f / 255.0f);
+                const bool upd1 = jpos < last1 && !(power.y > 0.0f) && !(a1 < 1.0f / 255.0f);
+                if (jpos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, upd0 || upd1)) continue;   // warp-uniform
+                const float2 aT = mul2(make_float2(upd0 ? a0 : 0.f, upd1 ? a1 : 0.f), T);
+                T = make_float2(upd0 ? test_T.x : T.x, upd1 ? test_T.y : T.y);
+                const float2 c0 = mul2(aT, dL0), c1 = mul2(aT, dL1), c2 = mul2(aT, dL2);
+                const float v = butterfly3(c0.x + c0.y, c1.x + c1.y, c2.x + c2.y, lane);
+                if (owner) atomicAdd(p.dL_dcolor + 3 * (size_t)s_id[j] + comp, v);
+            }
+        }
+    }
+}
+
+int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im, int ty0,
+                             int ty1, cudaStream_t s) {
+    ColorGradParams p;
+    p.W = a.W; p.H = a.H; p.grid_x = tiles_x(a.W); p.ty0 = ty0;
+    p.ranges = im.ranges; p.point_list = b.point_list;
+    p.subpixel_offset = reinterpret_cast<const float2*>(a.subpixel_offset);
+    p.rec = g.rec; p.n_contrib = im.n_contrib; p.blend_mask = im.blend_mask;
+    p.dL_dpix = a.dL_dpix; p.dL_dcolor = a.dL_dcolor;
+    if (ty1 <= ty0) return 0;
+    dim3 grid(p.grid_x, ty1 - ty0, 1);
+    render_color_grad_kernel<<<grid, 128, 0, s>>>(p);
+    count_launches(1);
+    return 0;
+}
+
 int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, int ty0, int ty1, cudaStream_t s) {
     RenderFwdParams p;

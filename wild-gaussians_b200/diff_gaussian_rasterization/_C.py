@@ -108,8 +108,11 @@ def _load():
     lib.gsr_appearance_colors_forward.argtypes = [POINTER(GsrAppearanceArgs), c_void_p]
     lib.gsr_appearance_colors_backward.argtypes = [POINTER(GsrAppearanceArgs), c_void_p]
     lib.gsr_appearance_unpack_grads.argtypes = [c_void_p] * 11
+    lib.gsr_appearance_embedding_backward.argtypes = [POINTER(GsrAppearanceArgs), c_void_p]
+    lib.gsr_backward_colors.argtypes = [POINTER(GsrBackwardArgs), c_void_p]
+    lib.gsr_backward_colors.restype = c_int
     for name in ("gsr_appearance_pack_weights", "gsr_appearance_colors_forward", "gsr_appearance_colors_backward",
-                 "gsr_appearance_unpack_grads"):
+                 "gsr_appearance_unpack_grads", "gsr_appearance_embedding_backward"):
         getattr(lib, name).restype = c_int
     lib.gsr_gaussian_activations_forward.argtypes = [c_int] + [c_void_p] * 8
     lib.gsr_gaussian_activations_forward.restype = c_int

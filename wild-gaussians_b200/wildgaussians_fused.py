@@ -21,7 +21,9 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``,
 ``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187), and
 ``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
-after the last block asked for, fused attention).
+after the last block asked for, fused attention).  ``enable_method(method)`` does what ``enable`` does for
+``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
+through ``fused_embedding``.
 Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
 ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features); anything else falls through to the original
 method, so ``enable`` is always safe.
@@ -303,3 +305,24 @@ def disable(model):
             if hasattr(getattr(m, name, None), "__wrapped__"):
                 setattr(m, name, getattr(m, name).__wrapped__)
     return model
+
+
+def optimize_embedding(method, dataset, *, embedding=None):
+    """``WildGaussians.optimize_embedding`` on one geometry pass (``fused_embedding``); unsupported configurations run
+    the method's own implementation."""
+    import fused_embedding
+    return fused_embedding.optimize_embedding(method, dataset, embedding=embedding)
+
+
+def enable_method(method, **kw):
+    """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
+    ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged."""
+    enable(method.model, **kw)
+    method.optimize_embedding = types.MethodType(optimize_embedding, method)
+    return method
+
+
+def disable_method(method):
+    method.__dict__.pop("optimize_embedding", None)
+    disable(method.model)
+    return method
