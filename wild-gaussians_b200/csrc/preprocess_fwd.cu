@@ -241,6 +241,11 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const __grid_consta
             const float tau = logf(255.0f * op) * 1.0001f + 1e-4f;
             hx = sqrtf(2.f * tau * cov.x) * 1.0001f + 0.05f;
             hy = sqrtf(2.f * tau * cov.z) * 1.0001f + 0.05f;
+            // The composite evaluates the fp32 conic, not Sigma^-1.  For a nearly singular 2D covariance (a needle
+            // without a low-pass filter) the conic's small eigenvalue carries no correct digits and its alpha >= 1/255
+            // region reaches far beyond Sigma's box: no box then (the ellipse test on the conic still applies).
+            const double cdet = (double)conic.x * conic.z - (double)conic.y * conic.y;
+            if (!(cdet > 1e-3 * ((double)conic.x * conic.z))) { hx = 1e30f; hy = 1e30f; }
         }
         p.rec[2 * (size_t)idx + 0] = make_float4(point_image.x, point_image.y, hx, hy);
         p.rec[2 * (size_t)idx + 1] = make_float4(conic.x, conic.y, conic.z, op);
