@@ -318,6 +318,20 @@ int gsr_gaussian_activations_backward(int P, const float* scales_raw, const floa
                                       const float* dL_drotations, float* dL_dscales_raw, float* dL_dopacities_raw,
                                       float* dL_drotations_raw, void* stream);
 
+/* -- SH colours of models without appearance (optional entry points) ---------------------------------------------------
+ * The colour statements of GaussianModel._render_internal for appearance_enabled = False (wildgaussians/method.py:1555-1565)
+ * in one kernel per direction: colors = clamp_min(eval_sh(sh_degree, clamp_max(cat(features_dc, features_rest), 1),
+ * normalize(means3D - campos)) + 0.5, 0).  Storage degree 3: features_dc [P,3] and features_rest [P,45] (coefficient-major
+ * (k, channel), 16-byte aligned) raw and unclamped; sh_degree is the ACTIVE degree 0..3.  means3D [P,3], campos [3],
+ * colors [P,3], all fp32.  The backward recomputes the forward; dL_dcolors may be NULL (treated as zero).  It writes every
+ * entry of dL_dfeatures_dc [P,3], dL_dfeatures_rest [P,45] (16-byte aligned; zero above the active degree) and
+ * dL_dmeans3D [P,3] (through the view direction).  P = 0 is valid.                                                      */
+int gsr_sh_colors_forward(int P, int sh_degree, const float* features_dc, const float* features_rest, const float* means3D,
+                          const float* campos, float* colors, void* stream);
+int gsr_sh_colors_backward(int P, int sh_degree, const float* features_dc, const float* features_rest, const float* means3D,
+                           const float* campos, const float* dL_dcolors, float* dL_dfeatures_dc, float* dL_dfeatures_rest,
+                           float* dL_dmeans3D, void* stream);
+
 /* -- densification statistics (SURVEY.md 8f-4; optional entry point) -----------------------------------------------------
  * One pass over the Gaussians replacing wildgaussians/method.py:1997-1998 + GaussianModel.add_densification_stats
  * (:1470-1477): for every Gaussian with radii > 0: max_radii2D = max(., radii); xyz_grad += |grad.xy|;

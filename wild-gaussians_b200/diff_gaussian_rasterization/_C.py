@@ -118,6 +118,10 @@ def _load():
     lib.gsr_gaussian_activations_forward.restype = c_int
     lib.gsr_gaussian_activations_backward.argtypes = [c_int] + [c_void_p] * 11
     lib.gsr_gaussian_activations_backward.restype = c_int
+    lib.gsr_sh_colors_forward.argtypes = [c_int, c_int] + [c_void_p] * 6
+    lib.gsr_sh_colors_forward.restype = c_int
+    lib.gsr_sh_colors_backward.argtypes = [c_int, c_int] + [c_void_p] * 9
+    lib.gsr_sh_colors_backward.restype = c_int
     lib.gsr_densification_stats.argtypes = [c_int] + [c_void_p] * 8
     lib.gsr_densification_stats.restype = c_int
     lib.gsr_adam_step.argtypes = [POINTER(GsrAdamSegment), c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_int, c_void_p]

@@ -9,6 +9,9 @@ the activations never leave the SM.  Opt-in: ``wildgaussians/method.py`` itself 
 
 Shapes are those of the reference's default config (config.py:16,49,59): SH degree 3 storage (3 + 45 features),
 24 per-Gaussian embedding features (6 x appearance_n_fourier_freqs), 32-d image embedding, hidden width 128.
+``fused_sh_colors(...)`` is the colour op of models without appearance (method.py:1555-1565, ``csrc/sh_colors.cu``):
+the raw SH colours alone, one bandwidth-bound kernel per direction.  ``fused_activations(...)`` is ``get_gaussians``
+without its features part (``csrc/activations.cu``).
 There is no PyTorch fallback: other shapes raise.
 """
 from __future__ import annotations
@@ -147,9 +150,59 @@ class _FusedActivations(torch.autograd.Function):
         return ds, do, dr, None
 
 
+def _aligned16(t):
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+class _FusedSHColors(torch.autograd.Function):
+    """The SH colours of a model without appearance (method.py:1555-1565, ``csrc/sh_colors.cu``): one kernel per direction."""
+
+    @staticmethod
+    def forward(ctx, features_dc, features_rest, means3D, campos, active_sh_degree):
+        dev = features_dc.device
+        P = int(features_dc.shape[0])
+        if not all(t.is_cuda for t in (features_dc, features_rest, means3D, campos)):
+            raise RuntimeError("fused_sh_colors needs CUDA tensors; there is no CPU path")
+        if (tuple(features_dc.shape) != (P, 3) or tuple(features_rest.shape) != (P, 45) or tuple(means3D.shape) != (P, 3)
+                or campos.numel() != 3 or not 0 <= int(active_sh_degree) <= 3):
+            raise RuntimeError("fused_sh_colors supports SH degree 3 storage only: features_dc [P,3], features_rest [P,45], "
+                               "means3D [P,3], campos [3], active degree 0..3")
+        fdc, frest, means, cam = (_f32c(t.detach()) for t in (features_dc, features_rest, means3D, campos))
+        frest = _aligned16(frest)
+        deg = int(active_sh_degree)
+        with torch.cuda.device(dev):
+            colors = torch.empty((P, 3), dtype=torch.float32, device=dev)
+            _C._check(_lib.gsr_sh_colors_forward(P, deg, fdc.data_ptr(), frest.data_ptr(), means.data_ptr(), cam.data_ptr(),
+                                                 colors.data_ptr(), _stream(dev)), "gsr_sh_colors_forward")
+        ctx.save_for_backward(fdc, frest, means, cam)
+        ctx.deg = deg
+        return colors
+
+    @staticmethod
+    def backward(ctx, g_colors):
+        fdc, frest, means, cam = ctx.saved_tensors
+        dev = fdc.device
+        P = int(fdc.shape[0])
+        with torch.cuda.device(dev):
+            g = None if g_colors is None else _f32c(g_colors)
+            d_dc, d_rest, d_means = torch.empty_like(fdc), torch.empty_like(frest), torch.empty_like(means)
+            _C._check(_lib.gsr_sh_colors_backward(P, ctx.deg, fdc.data_ptr(), frest.data_ptr(), means.data_ptr(), cam.data_ptr(),
+                                                  None if g is None else g.data_ptr(), d_dc.data_ptr(), d_rest.data_ptr(),
+                                                  d_means.data_ptr(), _stream(dev)), "gsr_sh_colors_backward")
+        return d_dc, d_rest, d_means, None, None
+
+
 def fused_activations(scales_raw, opacities_raw, rotations_raw, filter_3D):
     """``(scales, opacities, rotations)`` as ``GaussianModel.get_gaussians`` returns them (method.py:1060-1086)."""
     return _FusedActivations.apply(scales_raw, opacities_raw, rotations_raw, filter_3D)
+
+
+def fused_sh_colors(features_dc, features_rest, means3D, campos, active_sh_degree):
+    """``colors [P,3]`` as ``GaussianModel._render_internal`` computes them for a model without appearance
+    (method.py:1555-1565): ``clamp_min(eval_sh(deg, clamp_max(cat(dc, rest), 1), normalize(means3D - campos)) + 0.5, 0)``.
+    The arguments are the model's raw parameters (unclamped, storage degree 3) and the camera centre; the gradient
+    reaches ``features_dc``, ``features_rest`` (zero above the active degree) and ``means3D``."""
+    return _FusedSHColors.apply(features_dc, features_rest, means3D, campos, int(active_sh_degree))
 
 
 def fused_colors(features_dc, features_rest, embeddings, app_embedding, mlp, means3D, campos, active_sh_degree,

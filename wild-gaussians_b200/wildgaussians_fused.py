@@ -10,6 +10,8 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 * evaluates the raw and the appearance-toned colours with ONE fused kernel per direction (``fused_colors``:
   wgmma MLP + SH evaluation, ``csrc/appearance.cu``) instead of ~60 PyTorch launches and several P x 128 / P x 48
   fp32 intermediates (method.py:1570-1598);
+* for a model without appearance, evaluates the SH colours with one bandwidth-bound kernel per direction
+  (``fused_sh_colors``, ``csrc/sh_colors.cu``) and composites once, as the reference does (method.py:1555-1583);
 * caches the per-camera constants -- the numpy 4x4 inversions, ``getWorld2View2``, the projection matrix, the camera
   centre, tan(fov) (method.py:1502-1527) -- per (pose, intrinsics, size), and the all-zero ``subpixel_offset`` /
   background tensors per (H, W, device): no per-call H2D copies, ``zeros(H, W, 2)`` fills or device-side 4x4 inverse;
@@ -24,9 +26,10 @@ into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (meth
 after the last block asked for, fused attention).  ``enable_method(method)`` does what ``enable`` does for
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
 through ``fused_embedding``.
-Only the reference's default configuration is accelerated (appearance on with separate tuned colour,
-``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features); anything else falls through to the original
-method, so ``enable`` is always safe.
+Two configurations are accelerated, which covers all three presets the reference ships: appearance on with separate
+tuned colour, ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features (the default, and the phototourism
+preset), and appearance off with SH degree 3 (the NeRF On-the-go preset; ``embedding`` is then ignored, as the
+reference ignores it).  Anything else falls through to the original method, so ``enable`` is always safe.
 """
 from __future__ import annotations
 
@@ -38,7 +41,7 @@ import numpy as np
 import torch
 
 from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer, _C
-from fused_colors import fused_activations, fused_colors
+from fused_colors import fused_activations, fused_colors, fused_sh_colors
 
 _cam_cache: dict = {}
 _zero_cache: dict = {}
@@ -93,6 +96,7 @@ def _active_degree(model) -> int:
 
 
 def _supported(model, config) -> bool:
+    """The appearance-on configuration the fused colour op covers (the reference's default)."""
     c = model.config
     return (bool(c.appearance_enabled) and bool(c.appearance_separate_tuned_color) and not bool(c.appearance_model_sh)
             and int(c.sh_degree) == 3 and model.features_rest is not None and model.embeddings is not None
@@ -100,10 +104,19 @@ def _supported(model, config) -> bool:
             and model.xyz.is_cuda and not bool(config.debug))
 
 
+def _supported_sh(model, config) -> bool:
+    """The appearance-off configuration (e.g. the NeRF On-the-go preset) that ``fused_sh_colors`` covers: SH degree 3
+    storage; storage degree 0 (no ``features_rest``) is a different branch of the reference and falls through."""
+    c = model.config
+    return (not bool(c.appearance_enabled) and int(c.sh_degree) == 3 and model.features_rest is not None
+            and model.xyz.is_cuda and not bool(config.debug))
+
+
 def render_internal(self, viewpoint_camera, config, *, kernel_size, scaling_modifier=1.0, embedding, return_raw=True,
                     render_depth=False):
     """Drop-in for ``GaussianModel._render_internal``: same arguments, same output dictionary."""
-    if embedding is None or not _supported(self, config):
+    appearance = embedding is not None and _supported(self, config)
+    if not (appearance or _supported_sh(self, config)):
         return type(self)._render_internal(self, viewpoint_camera, config, kernel_size=kernel_size,
                                            scaling_modifier=scaling_modifier, embedding=embedding, return_raw=return_raw,
                                            render_depth=render_depth)
@@ -131,16 +144,23 @@ def render_internal(self, viewpoint_camera, config, *, kernel_size, scaling_modi
     # activations + 3D filter (get_gaussians, method.py:1060-1086) in one kernel per direction
     means3D = self.xyz
     scales, opacity, rotations = fused_activations(self.scales, self.opacities, self.rotations, self.filter_3D)
-    colors_raw, colors_toned = fused_colors(self.features_dc, self.features_rest, self.embeddings, embedding,
-                                            self.appearance_mlp.mlp, means3D, cc["cam_center"], deg, want_raw=bool(return_raw))
     kw = dict(means3D=means3D, means2D=screenspace_points, opacities=opacity, scales=scales, rotations=rotations, shs=None,
               cov3D_precomp=None)
-    raw_image = radii = accumulation = None
-    if return_raw:
-        raw_image, radii, accumulation = rasterizer(colors_precomp=colors_raw, **kw)
-    image, radii2, accumulation2 = rasterizer(colors_precomp=colors_toned, **kw)
-    radii = radii2 if radii is None else radii
-    accumulation = accumulation2 if accumulation is None else accumulation
+    if appearance:
+        colors_raw, colors_toned = fused_colors(self.features_dc, self.features_rest, self.embeddings, embedding,
+                                                self.appearance_mlp.mlp, means3D, cc["cam_center"], deg,
+                                                want_raw=bool(return_raw))
+        raw_image = radii = accumulation = None
+        if return_raw:
+            raw_image, radii, accumulation = rasterizer(colors_precomp=colors_raw, **kw)
+        image, radii2, accumulation2 = rasterizer(colors_precomp=colors_toned, **kw)
+        radii = radii2 if radii is None else radii
+        accumulation = accumulation2 if accumulation is None else accumulation
+    else:
+        # no appearance model (method.py:1573-1583): one pass with the SH colours; `embedding` is ignored
+        colors = fused_sh_colors(self.features_dc, self.features_rest, means3D, cc["cam_center"], deg)
+        image, radii, accumulation = rasterizer(colors_precomp=colors, **kw)
+        raw_image = image
     out = {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
            "accumulation": accumulation, "radii": radii}
     if return_raw:
