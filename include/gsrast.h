@@ -418,6 +418,40 @@ int gsr_ssim_down_forward(int B, int H, int W, int h, int w, const float* img1, 
 size_t gsr_attention_scratch_bytes(int B, int N, int H);            /* 0 for invalid sizes */
 int gsr_attention_forward(int B, int N, int H, const float* qkv, float* out, void* scratch, void* stream);
 
+/* -- Head and `dino`-mode loss of the uncertainty model (optional entry points) -----------------------------------------
+ * After the frozen backbone: `_forward_uncertainty_features` (wildgaussians/method.py:300-323; dropout2d, BatchNorm in
+ * training mode, the 1x1 conv_seg, + log(e - 1), softplus, bilinear upsample, clamp, crop) and the `dino` branch of
+ * `_compute_losses` (:363-433) for batch 1, fp32, everything contiguous on the device.
+ *   feat: [C][th][tw] backbone features of the normalised, padded ground truth (padded size Hp x Wp, image H x W at
+ *   (pad_top, pad_left)); mask: [C] dropout2d channel scales (0 or 1 / (1 - p)); conv_w [C], conv_b [1], bn_w [C],
+ *   bn_b [C]: the head's parameters; running_mean / running_var [C] and num_batches_tracked (int64) are updated as
+ *   F.batch_norm in training mode does with exponential factor bn_momentum (any of the three may be NULL).
+ *   gt, pred: [3][H][W]; ssim, msssim: [H][W] (the statistics of method.py:368-369).  (nh, nw): the 350-px map size
+ *   (dino_downsample; == (H, W) without a resize); feat_gt_down, feat_pred_down: [C][ch][cw] features of the two 350-px
+ *   images, padded to nHp x nWp with the map at (npad_top, npad_left).
+ *   Outputs: loss_mult [H][W] (min(1 / (2 u^2), 3)); loss [1]; metrics [7]: loss, ssim, msssim, ssim_discounted,
+ *   mse_discounted, psnr_discounted, beta.  scratch: gsr_uncertainty_scratch_bytes bytes of device memory, kept
+ *   unchanged from a forward to its backward.  The backward takes dL_dloss [1] and writes d_conv_w, d_conv_b, d_bn_w,
+ *   d_bn_b (the backbone features take no gradient).  Six launches forward, three backward; no atomics, no host
+ *   synchronisation; 1 <= C <= 2048, th * tw >= 2.                                                                         */
+typedef struct GsrUncertaintyArgs {
+    int C, th, tw, Hp, Wp, pad_top, pad_left, H, W;
+    int nh, nw, ch, cw, nHp, nWp, npad_top, npad_left;
+    float clip_min, reg_weight, bn_eps, bn_momentum;
+    const float *feat, *feat_gt_down, *feat_pred_down, *mask;
+    const float *conv_w, *conv_b, *bn_w, *bn_b;
+    float *running_mean, *running_var;
+    long long* num_batches_tracked;
+    const float *gt, *pred, *ssim, *msssim;
+    float *loss_mult, *loss, *metrics;
+    void* scratch;
+    const float* dL_dloss;
+    float *d_conv_w, *d_conv_b, *d_bn_w, *d_bn_b;
+} GsrUncertaintyArgs;
+size_t gsr_uncertainty_scratch_bytes(const GsrUncertaintyArgs* args);   /* 0 for invalid sizes */
+int gsr_uncertainty_forward(const GsrUncertaintyArgs* args, void* stream);
+int gsr_uncertainty_backward(const GsrUncertaintyArgs* args, void* stream);
+
 /* Optional per-stage device timing (cudaEvents on the caller's stream around each stage of the
  * next forward / backward calls).  The caller synchronises the stream, then reads the stage times of
  * the most recent calls in milliseconds (-1 for stages that did not run).  Not thread-safe.        */

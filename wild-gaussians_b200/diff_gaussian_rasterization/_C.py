@@ -68,6 +68,16 @@ class GsrAdamSegment(Structure):      # include/gsrast.h
 ADAM_MAX_SEGMENTS = 32
 
 
+class GsrUncertaintyArgs(Structure):      # include/gsrast.h
+    _fields_ = ([(n, c_int) for n in ("C", "th", "tw", "Hp", "Wp", "pad_top", "pad_left", "H", "W", "nh", "nw", "ch", "cw",
+                                      "nHp", "nWp", "npad_top", "npad_left")] +
+                [(n, c_float) for n in ("clip_min", "reg_weight", "bn_eps", "bn_momentum")] +
+                [(n, c_void_p) for n in ("feat", "feat_gt_down", "feat_pred_down", "mask", "conv_w", "conv_b", "bn_w", "bn_b",
+                                         "running_mean", "running_var", "num_batches_tracked", "gt", "pred", "ssim", "msssim",
+                                         "loss_mult", "loss", "metrics", "scratch", "dL_dloss", "d_conv_w", "d_conv_b",
+                                         "d_bn_w", "d_bn_b")])
+
+
 class GsrStats(Structure):
     _fields_ = [("num_rendered", c_int), ("num_visible", c_int), ("num_tiles", c_int), ("num_coarse", c_int)]
 
@@ -150,6 +160,12 @@ def _load():
     lib.gsr_attention_scratch_bytes.restype = c_size_t
     lib.gsr_attention_forward.argtypes = [c_int] * 3 + [c_void_p] * 4
     lib.gsr_attention_forward.restype = c_int
+    lib.gsr_uncertainty_scratch_bytes.argtypes = [POINTER(GsrUncertaintyArgs)]
+    lib.gsr_uncertainty_scratch_bytes.restype = c_size_t
+    lib.gsr_uncertainty_forward.argtypes = [POINTER(GsrUncertaintyArgs), c_void_p]
+    lib.gsr_uncertainty_forward.restype = c_int
+    lib.gsr_uncertainty_backward.argtypes = [POINTER(GsrUncertaintyArgs), c_void_p]
+    lib.gsr_uncertainty_backward.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

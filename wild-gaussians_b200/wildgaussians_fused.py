@@ -23,7 +23,8 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``,
 ``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187), and
 ``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
-after the last block asked for, fused attention).  ``enable_method(method)`` does what ``enable`` does for
+after the last block asked for, fused attention), and ``enable(model, uncertainty=True)`` the uncertainty model's
+``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits).  ``enable_method(method)`` does what ``enable`` does for
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
 through ``fused_embedding``.
 Two configurations are accelerated, which covers all three presets the reference ships: appearance on with separate
@@ -275,7 +276,18 @@ def dino_get_intermediate_layers(self, x, n=1, reshape=False, return_class_token
     return type(self).get_intermediate_layers(self, x, n, reshape, return_class_token, norm)
 
 
-def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False):
+def uncertainty_compute_losses(self, gt, prediction, prefix='', _cache_entry=None):
+    """Drop-in for ``UncertaintyModel._compute_losses`` (method.py:363-433): ``fused_uncertainty`` where it supports the
+    call (``dino`` mode, batch 1, fp32 on the GPU, training mode, no cross-process BatchNorm), the class's own method
+    otherwise."""
+    import fused_uncertainty
+    if fused_uncertainty.supported(self, gt, prediction):
+        return fused_uncertainty.compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
+    return type(self)._compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
+
+
+def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False,
+           uncertainty: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -284,7 +296,10 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     ``msssim`` and ``ssim_down`` (the uncertainty loss, method.py:360, :368-369, :407) are rebound to ``fused_ssim.msssim``
     and ``fused_ssim.ssim_down`` for supported input.  Those names are shared by every model of the module; ``disable``
     restores the originals.  With ``dino``, ``model.uncertainty_model.backbone.get_intermediate_layers`` (every DINOv2
-    call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``."""
+    call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``.
+    With ``uncertainty``, ``model.uncertainty_model._compute_losses`` (reached from ``get_loss``) is rebound, as an
+    instance attribute, to ``uncertainty_compute_losses``: the fused head and ``dino``-mode loss with a feature cache
+    that hits."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
@@ -304,6 +319,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     backbone = _dino_backbone(model)
     if dino and backbone is not None and "get_intermediate_layers" not in backbone.__dict__:
         backbone.get_intermediate_layers = types.MethodType(dino_get_intermediate_layers, backbone)
+    um = getattr(model, "uncertainty_model", None)
+    if uncertainty and um is not None and "_compute_losses" not in um.__dict__:
+        um._compute_losses = types.MethodType(uncertainty_compute_losses, um)
     return model
 
 
@@ -317,6 +335,9 @@ def disable(model):
     backbone = _dino_backbone(model)
     if backbone is not None:
         backbone.__dict__.pop("get_intermediate_layers", None)
+    um = getattr(model, "uncertainty_model", None)
+    if um is not None:
+        um.__dict__.pop("_compute_losses", None)
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
     m = sys.modules.get(type(model).__module__)
