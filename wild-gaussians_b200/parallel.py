@@ -42,11 +42,23 @@ def partition_tile_rows(num_tile_rows: int, world_size: int, weights: Sequence[f
     total = cum[-1]
     cuts = [0]
     for r in range(1, w):
-        # first row boundary at which the running weight reaches r/w of the total
-        e = bisect.bisect_left(cum, total * r / w - 1e-9 * max(1.0, total))
+        # first row boundary at which the running weight reaches r/w of the total; the rounding slack is relative, so
+        # tiny totals do not pull every cut down to row 0
+        e = bisect.bisect_left(cum, total * r / w - 1e-9 * total)
         cuts.append(min(n, max(e, cuts[-1])))
     cuts.append(n)
     return [(cuts[r], cuts[r + 1]) for r in range(w)]
+
+
+def abi_band(band: Tuple[int, int], H: int) -> Tuple[int, int]:
+    """A rank's band as the ``_C`` calls take it.  There ``(0, 0)`` is the single-GPU "whole image" shard, so an empty
+    band -- ``(0, 0)`` included -- is handed over as the empty band below the last tile row; otherwise a rank without
+    rows would composite the whole image and add its sums on top of everyone else's."""
+    y0, y1 = int(band[0]), int(band[1])
+    if y1 <= y0:
+        gy = (int(H) + TILE - 1) // TILE
+        return gy, gy
+    return y0, y1
 
 
 def band_pixel_rows(band: Tuple[int, int], H: int) -> Tuple[int, int]:
@@ -182,7 +194,7 @@ def sharded_forward(fwd_args, bands, group=None):
     rank = dist.get_rank(group)
     means3D = fwd_args[1]
     P, H, W = int(means3D.size(0)), int(fwd_args[14]), int(fwd_args[15])
-    shard = tuple(bands[rank])
+    shard = abi_band(bands[rank], H)
     st = _peers(P, H, W, means3D.device, group)
     if st is not None:
         image, hdl = st.images[st.frame], st.image_hdls[st.frame]
@@ -226,10 +238,10 @@ def sharded_backward(bwd_args, bands, group=None):
     from diff_gaussian_rasterization import _C
     rank = dist.get_rank(group)
     means3D = bwd_args[1]
-    shard = tuple(bands[rank])
+    H, W = int(bwd_args[14].size(1)), int(bwd_args[14].size(2))
+    shard = abi_band(bands[rank], H)
     if peer_mode(group) == 3:
         P = int(means3D.size(0))
-        H, W = int(bwd_args[14].size(1)), int(bwd_args[14].size(2))
         st = _peers(P, H, W, means3D.device, group)
         if st is not None and st.marks:
             # pull mode: local sums + marks, one barrier, then every rank reads the rows the others marked (no remote
