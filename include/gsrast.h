@@ -393,6 +393,35 @@ int gsr_ssim_forward(int B, int H, int W, const float* img1, const float* img2, 
 int gsr_ssim_backward(int B, int H, int W, const float* img1, const float* img2, const float* partials, const float* dL_dmap,
                       float* dL_dimg1, void* stream);
 
+/* -- loss block of the training step (optional entry points) -----------------------------------------------------------
+ * wildgaussians/method.py:1920-1992 around the SSIM: scale_grads by the mask and loss_mult, l1_loss, the weighted loss
+ * means and the metric sums.  toned, raw, gt: [3][H][W] fp32; mask, weight, grad_scale: [H][W] or NULL (mask NULL: no
+ * mask; weight NULL: loss_mult 1 in the loss; grad_scale NULL: no scale_grads by loss_mult).  raw_scaled [3][H][W]:
+ * raw after scale_grads, required when mask or grad_scale is given (it is the SSIM's input).  ssim_map [H][W],
+ * ssim_partials [9][H][W] (NULL when no backward follows): the buffers of gsr_ssim_forward, which the forward calls.
+ * c_l1 = fp32(1 - lambda_dssim), c_ssim = fp32(lambda_dssim).  Forward outputs: loss [1] (without the uncertainty
+ * term); metrics [8]: means of L1, SSIM and MSE, psnr, then with a mask mean(mask), sum(ssim m) / sum(m),
+ * sum(mse m) / sum(m), sum(L1 m) / sum(m) (zeros without a mask).  scratch: gsr_train_loss_scratch_bytes() bytes of
+ * device memory, 16-byte aligned.  The backward takes dL_dloss [1] and writes dL_dmap [H][W] (a scratch map),
+ * d_toned and d_raw [3][H][W].  Three launches forward, two backward; no float atomics, no host synchronisation.       */
+typedef struct GsrTrainLossArgs {
+    int H, W;
+    float c_l1, c_ssim;
+    const float *toned, *raw, *gt, *mask, *weight, *grad_scale;
+    float *raw_scaled, *ssim_map, *ssim_partials, *loss, *metrics;
+    void* scratch;
+    const float* dL_dloss;
+    float *dL_dmap, *d_toned, *d_raw;
+} GsrTrainLossArgs;
+size_t gsr_train_loss_scratch_bytes(void);
+int gsr_train_loss_forward(const GsrTrainLossArgs* args, void* stream);
+int gsr_train_loss_backward(const GsrTrainLossArgs* args, void* stream);
+/* Byte-staged training images: img_hwc [H][W][3] uint8 -> img_chw [3][H][W] fp32 and mask_hw [H][W] uint8 -> mask_out
+ * [H][W] fp32, each as x / 255.0f (IEEE division: the bits of numpy's astype(float32) / 255.0).  Either input may be
+ * NULL (not both).  One launch.                                                                                          */
+int gsr_unpack_u8(int H, int W, const unsigned char* img_hwc, const unsigned char* mask_hw, float* img_chw, float* mask_out,
+                  void* stream);
+
 /* -- Image-quality statistics of the uncertainty loss (optional entry points, forward only) -----------------------------
  * `msssim(x, y, max_size, min_size)` and `ssim_down(x, y, max_size)` of wildgaussians/method.py:126-187.  img1, img2:
  * [B,3,H,W] fp32, contiguous, on the device; out: [B,H,W].  (h, w) is the area-resize size the caller computed with

@@ -78,9 +78,13 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_fwd_kernel(int H, int W, co
     }
 }
 
+// SCALED: the result is multiplied per pixel by s0 then s1 ([B,H,W] each, NULL = 1), the backward of scale_grads on img1
+// (train_loss.cu); without it the kernel is the plain SSIM backward.
+template <bool SCALED>
 __global__ void __launch_bounds__(SSIM_THREADS) ssim_bwd_kernel(int H, int W, const float* __restrict__ img1,
                                                                 const float* __restrict__ img2, const float* __restrict__ partials,
                                                                 const float* __restrict__ dL_dmap, float* __restrict__ dL_dimg1,
+                                                                const float* __restrict__ s0, const float* __restrict__ s1,
                                                                 const SsimWindow win) {
     __shared__ float sf[3][SSIM_RH][SSIM_RW];
     __shared__ float hb[3][SSIM_RH][SSIM_TW];
@@ -135,7 +139,13 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_bwd_kernel(int H, int W, co
                 d2 = fmaf(w, hb[2][r + k][q], d2);
             }
             const size_t p = plane + (size_t)gy * W + gx;
-            dL_dimg1[p] = d0 + 2.f * img1[p] * d1 + img2[p] * d2;
+            float v = d0 + 2.f * img1[p] * d1 + img2[p] * d2;
+            if (SCALED) {
+                const size_t q = (size_t)b * HW + (size_t)gy * W + gx;
+                if (s0) v = __fmul_rn(v, s0[q]);
+                if (s1) v = __fmul_rn(v, s1[q]);
+            }
+            dL_dimg1[p] = v;
         }
     }
 }
@@ -143,6 +153,20 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_bwd_kernel(int H, int W, co
 static int ssim_check_sizes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) { set_error("bad sizes B=%d H=%d W=%d", B, H, W); return GSR_E_INVALID; }
     if (B > 65535 || (H + SSIM_TH - 1) / SSIM_TH > 65535) { set_error("image batch or height too large (B=%d H=%d)", B, H); return GSR_E_INVALID; }
+    return 0;
+}
+
+int ssim_backward_launch(int B, int H, int W, const float* img1, const float* img2, const float* partials,
+                         const float* dL_dmap, float* dL_dimg1, const float* s0, const float* s1, cudaStream_t stream) {
+    static const SsimWindow win = ssim_window();
+    if (s0 || s1)
+        ssim_bwd_kernel<true><<<ssim_grid(B, H, W), SSIM_THREADS, 0, stream>>>(H, W, img1, img2, partials, dL_dmap, dL_dimg1,
+                                                                              s0, s1, win);
+    else
+        ssim_bwd_kernel<false><<<ssim_grid(B, H, W), SSIM_THREADS, 0, stream>>>(H, W, img1, img2, partials, dL_dmap, dL_dimg1,
+                                                                               nullptr, nullptr, win);
+    count_launches(1);
+    GSR_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -168,9 +192,5 @@ extern "C" int gsr_ssim_backward(int B, int H, int W, const float* img1, const f
         set_error("img1, img2, partials, dL_dmap or dL_dimg1 is NULL");
         return GSR_E_INVALID;
     }
-    static const SsimWindow win = ssim_window();
-    ssim_bwd_kernel<<<ssim_grid(B, H, W), SSIM_THREADS, 0, (cudaStream_t)stream>>>(H, W, img1, img2, partials, dL_dmap, dL_dimg1, win);
-    count_launches(1);
-    GSR_CUDA(cudaGetLastError());
-    return 0;
+    return ssim_backward_launch(B, H, W, img1, img2, partials, dL_dmap, dL_dimg1, nullptr, nullptr, (cudaStream_t)stream);
 }

@@ -92,4 +92,8 @@ static dim3 ssim_grid(int B, int H, int W) {
     return dim3((W + SSIM_TW - 1) / SSIM_TW, (H + SSIM_TH - 1) / SSIM_TH, B);
 }
 
+// The SSIM backward (ssim.cu) on checked sizes, optionally scaled per pixel by s0 then s1 ([B,H,W], NULL = 1).
+int ssim_backward_launch(int B, int H, int W, const float* img1, const float* img2, const float* partials,
+                         const float* dL_dmap, float* dL_dimg1, const float* s0, const float* s1, cudaStream_t stream);
+
 }  // namespace gsr

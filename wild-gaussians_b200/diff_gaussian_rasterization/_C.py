@@ -78,6 +78,13 @@ class GsrUncertaintyArgs(Structure):      # include/gsrast.h
                                          "d_bn_w", "d_bn_b")])
 
 
+class GsrTrainLossArgs(Structure):      # include/gsrast.h
+    _fields_ = ([("H", c_int), ("W", c_int), ("c_l1", c_float), ("c_ssim", c_float)] +
+                [(n, c_void_p) for n in ("toned", "raw", "gt", "mask", "weight", "grad_scale", "raw_scaled", "ssim_map",
+                                         "ssim_partials", "loss", "metrics", "scratch", "dL_dloss", "dL_dmap", "d_toned",
+                                         "d_raw")])
+
+
 class GsrStats(Structure):
     _fields_ = [("num_rendered", c_int), ("num_visible", c_int), ("num_tiles", c_int), ("num_coarse", c_int)]
 
@@ -166,6 +173,14 @@ def _load():
     lib.gsr_uncertainty_forward.restype = c_int
     lib.gsr_uncertainty_backward.argtypes = [POINTER(GsrUncertaintyArgs), c_void_p]
     lib.gsr_uncertainty_backward.restype = c_int
+    lib.gsr_train_loss_scratch_bytes.argtypes = []
+    lib.gsr_train_loss_scratch_bytes.restype = c_size_t
+    lib.gsr_train_loss_forward.argtypes = [POINTER(GsrTrainLossArgs), c_void_p]
+    lib.gsr_train_loss_forward.restype = c_int
+    lib.gsr_train_loss_backward.argtypes = [POINTER(GsrTrainLossArgs), c_void_p]
+    lib.gsr_train_loss_backward.restype = c_int
+    lib.gsr_unpack_u8.argtypes = [c_int, c_int] + [c_void_p] * 5
+    lib.gsr_unpack_u8.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

@@ -35,7 +35,7 @@ import torch.nn.functional as F
 
 from diff_gaussian_rasterization import _C
 
-__all__ = ["compute_losses", "supported"]
+__all__ = ["compute_losses", "compute_losses_on_device", "supported"]
 
 _lib = _C._lib
 DINO_MAX_SIZE = 350                               # method.py:386-387
@@ -51,7 +51,7 @@ def _distributed_bn(bn) -> bool:
     return dist.get_world_size(group) > 1
 
 
-def _unsupported(model, gt, prediction) -> str | None:
+def _unsupported_model(model) -> str | None:
     cfg = model.config
     if cfg.uncertainty_mode != "dino":
         return "covers uncertainty_mode 'dino' only"
@@ -59,12 +59,20 @@ def _unsupported(model, gt, prediction) -> str | None:
         return "covers uncertainty_dino_max_size None only"
     if not model.training:
         return "covers training mode only"
-    bn, conv = model.bn, model.conv_seg
+    bn = model.bn
     if not (bn.training and bn.track_running_stats and bn.affine and bn.momentum is not None
             and bn.running_mean is not None and bn.num_batches_tracked is not None):
         return "needs a BatchNorm in training mode with affine parameters and running statistics"
     if _distributed_bn(bn):
         return "does not synchronise BatchNorm statistics across processes"
+    return None
+
+
+def _unsupported(model, gt, prediction) -> str | None:
+    why = _unsupported_model(model)
+    if why is not None:
+        return why
+    bn, conv = model.bn, model.conv_seg
     if not (isinstance(gt, torch.Tensor) and isinstance(prediction, torch.Tensor)):
         return "expects tensors"
     if gt.dim() != 4 or gt.shape != prediction.shape or gt.shape[0] != 1 or gt.shape[1] != 3:
@@ -187,6 +195,16 @@ def head_loss(feat, feat_gt_down, feat_pred_down, mask, conv, bn, gt, prediction
 
 def compute_losses(model, gt, prediction, prefix="", _cache_entry=None):
     """Drop-in for ``UncertaintyModel._compute_losses`` on supported input; raises otherwise."""
+    loss, metrics_t, loss_mult = compute_losses_on_device(model, gt, prediction, _cache_entry)
+    with torch.cuda.device(gt.device):
+        values = metrics_t.tolist()
+    metrics = {f"{prefix}{k}": v for k, v in zip(METRICS, values)}
+    return loss, metrics, loss_mult
+
+
+def compute_losses_on_device(model, gt, prediction, _cache_entry=None):
+    """``compute_losses`` without its read-back: ``(loss, metrics, loss_mult)`` with ``metrics`` the [7] device tensor of
+    the values under ``METRICS``; nothing synchronises with the host.  Raises on unsupported input."""
     why = _unsupported(model, gt, prediction)
     if why is not None:
         raise RuntimeError("fused_uncertainty.compute_losses " + why)
@@ -212,7 +230,4 @@ def compute_losses(model, gt, prediction, prefix="", _cache_entry=None):
     loss, metrics_t, loss_mult = head_loss(feat, fgd, fpd, mask.reshape(C), model.conv_seg, model.bn, gt, prediction, _ssim,
                                            _msssim, (int(gt_down.shape[2]), int(gt_down.shape[3])), int(model.patch_size),
                                            cfg.uncertainty_clip_min, cfg.uncertainty_regularizer_weight)
-    with torch.cuda.device(gt.device):
-        values = metrics_t.tolist()
-    metrics = {f"{prefix}{k}": v for k, v in zip(METRICS, values)}
-    return loss, metrics, loss_mult
+    return loss, metrics_t, loss_mult

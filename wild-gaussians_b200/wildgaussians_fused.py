@@ -26,7 +26,9 @@ into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (meth
 after the last block asked for, fused attention), and ``enable(model, uncertainty=True)`` the uncertainty model's
 ``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits).  ``enable_method(method)`` does what ``enable`` does for
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
-through ``fused_embedding``.
+through ``fused_embedding``; ``enable_method(method, train=True)`` also routes ``method.train_iteration``
+(method.py:1880-2024) through ``fused_train``: the loss block and its metrics as kernels, training images staged as
+bytes in pinned memory, one metric read-back per step.
 Two configurations are accelerated, which covers all three presets the reference ships: appearance on with separate
 tuned colour, ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features (the default, and the phototourism
 preset), and appearance off with SH degree 3 (the NeRF On-the-go preset; ``embedding`` is then ignored, as the
@@ -355,15 +357,21 @@ def optimize_embedding(method, dataset, *, embedding=None):
     return fused_embedding.optimize_embedding(method, dataset, embedding=embedding)
 
 
-def enable_method(method, **kw):
+def enable_method(method, train: bool = False, **kw):
     """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
-    ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged."""
+    ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged.  With
+    ``train``, ``method.train_iteration`` is rebound (instance attribute) to ``fused_train.train_iteration``: its loss
+    always runs as the fused op, while the backbone, ``msssim`` and the uncertainty head follow their own flags."""
     enable(method.model, **kw)
     method.optimize_embedding = types.MethodType(optimize_embedding, method)
+    if train:
+        import fused_train
+        method.train_iteration = types.MethodType(fused_train.train_iteration, method)
     return method
 
 
 def disable_method(method):
     method.__dict__.pop("optimize_embedding", None)
+    method.__dict__.pop("train_iteration", None)
     disable(method.model)
     return method
