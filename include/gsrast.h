@@ -340,6 +340,55 @@ int gsr_sh_colors_backward(int P, int sh_degree, const float* features_dc, const
 int gsr_densification_stats(int P, const int* radii, const float* viewspace_grad, float* max_radii2D, float* xyz_grad,
                             float* xyz_gradient_accum_abs, float* xyz_gradient_accum_abs_max, float* denom, void* stream);
 
+/* -- densify_and_prune / reset_opacity (optional entry points) ---------------------------------------------------------------
+ * GaussianModel.densify_and_prune (wildgaussians/method.py:1420-1468, with _densify_and_clone / _densify_and_split /
+ * _densification_postfix / _prune_points) in two steps that share `scratch` (gsr_densify_scratch_bytes(P) bytes of device
+ * memory, 16-byte aligned, kept alive from the plan to the apply):
+ *   gsr_densify_plan  decides every row's fate -- clone, split and the final prune, on the reference's fp32 arithmetic,
+ *                     with Q = the reference's quantile(grads_abs, 1 - ratio) (linear interpolation) found by a radix
+ *                     select, for any P -- and writes GSR_DENSIFY_COUNTS words to the DEVICE array `counts`:
+ *                     [0] rows cloned, [1] rows split (S), [2] rows after the final prune (P'), [3] rows of the post-split
+ *                     set whose largest scale exceeds prune_max_scale, [4] split rows kept, [5] rows with |grad| >= max_grad,
+ *                     [6] the bits of Q (float; 0 when accum_abs is NULL), [7] 0.
+ *   gsr_densify_apply writes every dynamically sized tensor of P' rows in the reference's order -- survivors of the rows
+ *                     that were not split, clones, split copy 1, split copy 2 -- from its old rows.  `normals` is the
+ *                     [2S,3] standard-normal draw the reference makes for the split children (its normal
+ *                     sample over a [2S,3] mean), split copy c of the r-th split row takes row c S + r.
+ * Inputs: xyz_grad / denom / accum_abs [P] (accum_abs NULL when use_gof_abs_gradient is off), xyz [P,3], scales [P,3] (log),
+ * rotations [P,4] (unnormalised), opacities [P] (logit), fp32.  The thresholds are the reference's Python floats rounded to
+ * fp32 (as the reference's fp32 tensor comparisons round them): max_grad, clone_max_scale = percent_dense * extent,
+ * min_opacity, prune_max_scale = 0.1 * extent (used only when size_pruning != 0).  split_scale_mul = fp32(1 / fp32(0.8 N)).
+ * Segments: src [P, width] -> dst [P', width]; COPY: clones and split copies repeat the source row; ZERO_NEW: new rows are
+ * zero (Adam moments, densification buffers); XYZ / SCALES (width 3): the split copies' positions (rotated samples) and
+ * log(exp(s) / 1.6).  Element offsets are 64-bit.  1 <= P <= GSR_DENSIFY_MAX_P.                                          */
+#define GSR_DENSIFY_COUNTS 8
+#define GSR_DENSIFY_MAX_SEGMENTS 48
+#define GSR_DENSIFY_MAX_P 0x3FFFFFFF
+enum { GSR_DENSIFY_COPY = 0, GSR_DENSIFY_ZERO_NEW = 1, GSR_DENSIFY_XYZ = 2, GSR_DENSIFY_SCALES = 3 };
+typedef struct GsrDensifyArgs {
+    int P;
+    const float *xyz_grad, *denom, *accum_abs;
+    const float *xyz, *scales, *rotations, *opacities;
+    float max_grad, clone_max_scale, min_opacity, prune_max_scale;
+    int size_pruning;
+    float split_scale_mul;
+    void* scratch;
+    unsigned int* counts;
+    const float* normals;   /* apply only; may be NULL when S = 0 */
+} GsrDensifyArgs;
+typedef struct GsrDensifySegment {
+    const float* src;
+    float* dst;
+    int width;
+    int kind;
+} GsrDensifySegment;
+size_t gsr_densify_scratch_bytes(int P);   /* 0 for an invalid P */
+int gsr_densify_plan(const GsrDensifyArgs* args, void* stream);
+int gsr_densify_apply(const GsrDensifyArgs* args, const GsrDensifySegment* segments, int num_segments, void* stream);
+/* GaussianModel.reset_opacity (method.py:1249-1266): out[i] = logit(min(opacity_with_filter, 0.01) / coef) on the 3D-filtered
+ * scales, opacities [P] (logit), scales [P,3] (log), filter_3D [P]; out may not alias opacities.  P = 0 is valid.          */
+int gsr_reset_opacity(int P, const float* opacities, const float* scales, const float* filter_3D, float* out, void* stream);
+
 /* -- optimizer step (SURVEY.md 8f-4; optional entry point) ------------------------------------------------------------------
  * One launch replacing `self.model.optimizer.step()` (wildgaussians/method.py:2019) of the Adam optimizer built at
  * method.py:1033-1049 (lr per group, eps = 1e-15, weight_decay on the appearance-embedding table only; amsgrad /

@@ -68,6 +68,24 @@ class GsrAdamSegment(Structure):      # include/gsrast.h
 ADAM_MAX_SEGMENTS = 32
 
 
+class GsrDensifyArgs(Structure):      # include/gsrast.h
+    _fields_ = ([("P", c_int)] +
+                [(n, c_void_p) for n in ("xyz_grad", "denom", "accum_abs", "xyz", "scales", "rotations", "opacities")] +
+                [(n, c_float) for n in ("max_grad", "clone_max_scale", "min_opacity", "prune_max_scale")] +
+                [("size_pruning", c_int), ("split_scale_mul", c_float), ("scratch", c_void_p), ("counts", c_void_p),
+                 ("normals", c_void_p)])
+
+
+class GsrDensifySegment(Structure):   # include/gsrast.h
+    _fields_ = [("src", c_void_p), ("dst", c_void_p), ("width", c_int), ("kind", c_int)]
+
+
+DENSIFY_COUNTS = 8
+DENSIFY_MAX_SEGMENTS = 48
+DENSIFY_MAX_P = 0x3FFFFFFF
+DENSIFY_COPY, DENSIFY_ZERO_NEW, DENSIFY_XYZ, DENSIFY_SCALES = 0, 1, 2, 3
+
+
 class GsrUncertaintyArgs(Structure):      # include/gsrast.h
     _fields_ = ([(n, c_int) for n in ("C", "th", "tw", "Hp", "Wp", "pad_top", "pad_left", "H", "W", "nh", "nw", "ch", "cw",
                                       "nHp", "nWp", "npad_top", "npad_left")] +
@@ -143,6 +161,14 @@ def _load():
     lib.gsr_densification_stats.restype = c_int
     lib.gsr_adam_step.argtypes = [POINTER(GsrAdamSegment), c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_int, c_void_p]
     lib.gsr_adam_step.restype = c_int
+    lib.gsr_densify_scratch_bytes.argtypes = [c_int]
+    lib.gsr_densify_scratch_bytes.restype = c_size_t
+    lib.gsr_densify_plan.argtypes = [POINTER(GsrDensifyArgs), c_void_p]
+    lib.gsr_densify_plan.restype = c_int
+    lib.gsr_densify_apply.argtypes = [POINTER(GsrDensifyArgs), POINTER(GsrDensifySegment), c_int, c_void_p]
+    lib.gsr_densify_apply.restype = c_int
+    lib.gsr_reset_opacity.argtypes = [c_int] + [c_void_p] * 5
+    lib.gsr_reset_opacity.restype = c_int
     lib.gsr_filter3d_scratch_bytes.argtypes = [c_int]
     lib.gsr_filter3d_scratch_bytes.restype = c_size_t
     lib.gsr_compute_3d_filter.argtypes = [c_int, c_void_p, c_int, c_void_p, c_float, c_void_p, c_void_p, c_void_p]

@@ -28,8 +28,11 @@ protected-iteration detach, the densification block on the model's own methods, 
 * Metrics: one device vector, copied into pinned memory and read after one event synchronisation at the end of the step.
 
 Host synchronisations per ordinary step: that metric read-back, plus the rasterizer's instance-count read-back inside
-the render (which sizes its binning buffers; unchanged here).  Steps that densify, reset the opacity, raise the SH
-degree or recompute the 3D filter keep the reference's own synchronisations there.
+the render (which sizes its binning buffers; unchanged here).  Densification and the opacity reset call
+``model.densify_and_prune`` / ``model.reset_opacity``: with ``enable_method(method, train=True, densify=True)`` those are
+the ``fused_densify`` kernels (one count read-back per densifying step, any number of Gaussians), otherwise the
+reference's methods with their own synchronisations.  Steps that raise the SH degree or recompute the 3D filter keep
+the reference's synchronisations there.
 
 ``supported(method)`` tells which methods this covers; ``wildgaussians_fused.enable_method(method, train=True)`` binds
 it and falls back to the class's own ``train_iteration`` for the rest.

@@ -24,7 +24,9 @@ into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (meth
 ``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187), and
 ``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
 after the last block asked for, fused attention), and ``enable(model, uncertainty=True)`` the uncertainty model's
-``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits).  ``enable_method(method)`` does what ``enable`` does for
+``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits),
+and ``enable(model, densify=True)`` ``densify_and_prune`` and ``reset_opacity`` through ``fused_densify`` (one gather kernel
+into final-size tensors, a GPU quantile without torch's 2^24-element limit, one synchronisation).  ``enable_method(method)`` does what ``enable`` does for
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
 through ``fused_embedding``; ``enable_method(method, train=True)`` also routes ``method.train_iteration``
 (method.py:1880-2024) through ``fused_train``: the loss block and its metrics as kernels, training images staged as
@@ -288,8 +290,22 @@ def uncertainty_compute_losses(self, gt, prediction, prefix='', _cache_entry=Non
     return type(self)._compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
 
 
+def densify_and_prune(self, max_grad, min_opacity, extent, enable_size_pruning, skyradius=None):
+    """Drop-in for ``GaussianModel.densify_and_prune`` (method.py:1420-1468): ``fused_densify`` where it supports the
+    model, the class's own method otherwise."""
+    import fused_densify
+    return fused_densify.densify_and_prune(self, max_grad, min_opacity, extent, enable_size_pruning, skyradius=skyradius)
+
+
+def reset_opacity(self):
+    """Drop-in for ``GaussianModel.reset_opacity`` (method.py:1249-1278): ``fused_densify`` where it supports the model,
+    the class's own method otherwise."""
+    import fused_densify
+    return fused_densify.reset_opacity(self)
+
+
 def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False,
-           uncertainty: bool = False):
+           uncertainty: bool = False, densify: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -301,7 +317,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``.
     With ``uncertainty``, ``model.uncertainty_model._compute_losses`` (reached from ``get_loss``) is rebound, as an
     instance attribute, to ``uncertainty_compute_losses``: the fused head and ``dino``-mode loss with a feature cache
-    that hits."""
+    that hits.  With ``densify``, ``model.densify_and_prune`` and ``model.reset_opacity`` are rebound, as instance
+    attributes, to the ``fused_densify`` kernels (same results, one synchronisation per densification, any number of
+    Gaussians)."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
@@ -324,6 +342,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     um = getattr(model, "uncertainty_model", None)
     if uncertainty and um is not None and "_compute_losses" not in um.__dict__:
         um._compute_losses = types.MethodType(uncertainty_compute_losses, um)
+    if densify:
+        model.densify_and_prune = types.MethodType(densify_and_prune, model)
+        model.reset_opacity = types.MethodType(reset_opacity, model)
     return model
 
 
@@ -334,6 +355,8 @@ def _dino_backbone(model):
 def disable(model):
     model.__dict__.pop("_render_internal", None)
     model.__dict__.pop("compute_3D_filter", None)
+    model.__dict__.pop("densify_and_prune", None)
+    model.__dict__.pop("reset_opacity", None)
     backbone = _dino_backbone(model)
     if backbone is not None:
         backbone.__dict__.pop("get_intermediate_layers", None)
@@ -361,7 +384,8 @@ def enable_method(method, train: bool = False, **kw):
     """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
     ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged.  With
     ``train``, ``method.train_iteration`` is rebound (instance attribute) to ``fused_train.train_iteration``: its loss
-    always runs as the fused op, while the backbone, ``msssim`` and the uncertainty head follow their own flags."""
+    always runs as the fused op, while the backbone, ``msssim``, the uncertainty head and densification (``densify``)
+    follow their own flags."""
     enable(method.model, **kw)
     method.optimize_embedding = types.MethodType(optimize_embedding, method)
     if train:
