@@ -16,6 +16,10 @@ Bars.  The MLP runs with bf16 operands (fp32 accumulation); everything else is f
     exactly like any bf16 autocast training step -- differs from the fp32 network's by ~5 % in max-norm while
     agreeing in direction.  Against the fp32 / fp64 reference the test therefore asserts direction and size (cosine
     >= 0.99, norm ratio within 3 %) instead of an entry-wise bound.
+These bars pin the op to the reference goldens and to the fp32 network.  The entry-wise bars are in
+tests/test_colour_op_exact.py: every colour and every per-Gaussian gradient of every row, and every weight, bias and
+image-embedding gradient entry, within an a-priori bound of an fp64 oracle of the rounded network
+(oracle/color_exact.py), on lattice, random and golden scenes, at the tile / warpgroup / CTA-boundary shapes.
 """
 import os
 import sys
@@ -195,3 +199,38 @@ def test_fused_activations_against_torch_statements():
         assert float((a - b).abs().max()) < 1e-5 * max(1.0, float(b.abs().max()))
     for a, b in zip(res[0][1], res[1][1]):
         assert float((a - b).abs().max()) < 1e-4 * max(1.0, float(b.abs().max()))
+
+    # Edge rows, against the same statements in float64 and row by row (their gradients reach 1e12):
+    #  * quaternions below F.normalize's eps (|q| ~ 5.5e-13, and exactly 0): x / clamp_min(|x|, eps) has gradient g / eps
+    #    there, the clamp passing nothing to the norm -- not the projected (g - n (n.g)) / |q|;
+    #  * filter_3D == 0 with scale products in the fp32 denormal range (raw^2 ~ 1e-13 .. 1e-18): coef == 1 exactly, and
+    #    its gradient is 0 (the fp32 torch statements give NaN and -inf there: prod^2 underflows);
+    #  * saturated sigmoids (|opacity| = 40, 100).
+    s_e = torch.tensor([[-15.0, -15.0, -15.0], [-20.0, -14.0, -16.0], [-1.0, -2.0, -3.0], [-15.0, -1.0, -2.0],
+                        [-0.5, -0.7, -0.2], [-2.0, -2.0, -2.0]], device=dev)
+    o_e = torch.tensor([[40.0], [-40.0], [-100.0], [100.0], [0.3], [-1.0]], device=dev)
+    r_e = torch.tensor([[3e-13, -4e-13, 1e-13, 2e-13], [0.0, 0.0, 0.0, 0.0], [1.0, 2.0, 3.0, 4.0], [-1e-13, 0.0, 0.0, 0.0],
+                        [3.0, -4.0, 1.0, 2.0], [0.0, 0.0, 0.0, 7e-13]], device=dev)
+    f_e = torch.tensor([[0.0], [0.0], [0.0], [0.0], [1e-3], [0.0]], device=dev)
+    g_e = [torch.randn(*t.shape, generator=g).to(dev) for t in (s_e, o_e, r_e)]
+
+    def ref64(s, o, r):
+        f64 = f_e.double()
+        rot = torch.nn.functional.normalize(r)
+        raw = torch.exp(s)
+        scales = (torch.square(raw) + torch.square(f64)).sqrt()
+        coef = torch.sqrt(torch.square(raw).prod(dim=1) / (torch.square(raw) + torch.square(f64)).prod(dim=1))
+        return scales, torch.sigmoid(o) * coef[..., None], rot
+
+    res = []
+    for fn, dt in ((lambda a, b, c: fc.fused_activations(a, b, c, f_e), torch.float32), (ref64, torch.float64)):
+        L = [t.to(dt).clone().requires_grad_(True) for t in (s_e, o_e, r_e)]
+        out = fn(*L)
+        torch.autograd.backward(list(out), [t.to(dt) for t in g_e])
+        res.append(([x.detach().double() for x in out], [t.grad.double() for t in L]))
+    for a, b in zip(res[0][0], res[1][0]):
+        assert torch.isfinite(a).all()
+        assert bool(((a - b).abs() <= 1e-5 * b.abs().amax(1, keepdim=True).clamp_min(1.0)).all()), (a, b)
+    for a, b in zip(res[0][1], res[1][1]):
+        assert torch.isfinite(a).all()
+        assert bool(((a - b).abs() <= 1e-5 * b.abs().amax(1, keepdim=True) + 1e-12).all()), (a, b)

@@ -17,6 +17,7 @@ struct ActRow {
     float sig, coef;
     float4 q;                       // raw quaternion
     float inv_n;                    // 1 / max(|q|, 1e-12)
+    bool q_clamped;                 // |q| < 1e-12: F.normalize divides by the constant eps
 };
 
 __device__ __forceinline__ ActRow act_forward(const float* __restrict__ scales, const float* __restrict__ opac,
@@ -36,7 +37,9 @@ __device__ __forceinline__ ActRow act_forward(const float* __restrict__ scales, 
     r.coef = sqrtf(num / den);
     r.sig = 1.0f / (1.0f + expf(-opac[i]));
     r.q = rot[i];
-    r.inv_n = 1.0f / fmaxf(sqrtf(r.q.x * r.q.x + r.q.y * r.q.y + r.q.z * r.q.z + r.q.w * r.q.w), 1e-12f);
+    const float qn = sqrtf(r.q.x * r.q.x + r.q.y * r.q.y + r.q.z * r.q.z + r.q.w * r.q.w);
+    r.q_clamped = qn < 1e-12f;
+    r.inv_n = 1.0f / fmaxf(qn, 1e-12f);
     return r;
 }
 
@@ -71,6 +74,10 @@ __global__ void __launch_bounds__(256) activations_bwd_kernel(int P, const float
     }
     d_opac[i] = go * r.coef * r.sig * (1.0f - r.sig);
     float4 g = g_rot ? g_rot[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r.q_clamped) {      // x / clamp_min(|x|, eps): below eps the clamp passes no gradient to the norm
+        d_rot[i] = make_float4(g.x * r.inv_n, g.y * r.inv_n, g.z * r.inv_n, g.w * r.inv_n);
+        return;
+    }
     const float4 n = make_float4(r.q.x * r.inv_n, r.q.y * r.inv_n, r.q.z * r.inv_n, r.q.w * r.inv_n);
     const float d = g.x * n.x + g.y * n.y + g.z * n.z + g.w * n.w;
     d_rot[i] = make_float4((g.x - n.x * d) * r.inv_n, (g.y - n.y * d) * r.inv_n, (g.z - n.z * d) * r.inv_n, (g.w - n.w * d) * r.inv_n);

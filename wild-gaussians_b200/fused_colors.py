@@ -57,6 +57,7 @@ class _FusedColors(torch.autograd.Function):
         tens = [_f32c(t.detach()) for t in (features_dc, features_rest, embeddings, app_embedding, W1, b1, W2, b2, W3, b3,
                                             means3D, campos)]
         (fdc, frest, gemb, aemb, w1, bb1, w2, bb2, w3, bb3, means, cam) = tens
+        frest, gemb = _aligned16(frest), _aligned16(gemb)         # the kernels read them as 16-byte vectors
         with torch.cuda.device(dev):
             blob = torch.empty((_lib.gsr_appearance_packed_weight_bytes(),), dtype=torch.uint8, device=dev)
             _C._check(_lib.gsr_appearance_pack_weights(w1.data_ptr(), bb1.data_ptr(), w2.data_ptr(), bb2.data_ptr(), w3.data_ptr(),
