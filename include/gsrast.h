@@ -530,6 +530,27 @@ size_t gsr_uncertainty_scratch_bytes(const GsrUncertaintyArgs* args);   /* 0 for
 int gsr_uncertainty_forward(const GsrUncertaintyArgs* args, void* stream);
 int gsr_uncertainty_backward(const GsrUncertaintyArgs* args, void* stream);
 
+/* -- Evaluation metrics (optional entry points) ------------------------------------------------------------------------
+ * The per-image sums behind `compute_metrics` of wildgaussians/evaluation.py:331-352.  a, b: [B][H][W][C], each uint8
+ * (a_u8 != 0, read as v / 255.0f) or fp32, contiguous, on the device; both are clipped to [0, 1] as np.clip does it.
+ * taps: the 11 dm_pix Gaussian taps (sigma 1.5, as the host computes them); c1 = (k1 max_val)^2, c2 = (k2 max_val)^2.
+ * Outputs: sums [B][3] fp64: sum of (a - b)^2 and of |a - b| over all H W C values (fp32 terms), and sum of the SSIM
+ * map over its (H - 10) (W - 10) C valid outputs (filtered in fp64); lpips_a, lpips_b (both or neither): x * 2 - 1 of the
+ * clipped a and b, fp32 [B][H][W][C].  scratch: gsr_metrics_scratch_bytes bytes of device memory, 8-byte aligned.
+ * H >= 11, W >= 11, B * C <= 65535.  Two launches, no atomics, no host synchronisation.                               */
+typedef struct GsrMetricsArgs {
+    int B, H, W, C;
+    int a_u8, b_u8;
+    const void *a, *b;
+    double taps[11];
+    double c1, c2;
+    float *lpips_a, *lpips_b;
+    double* sums;
+    void* scratch;
+} GsrMetricsArgs;
+size_t gsr_metrics_scratch_bytes(int B, int H, int W, int C);   /* 0 for invalid sizes */
+int gsr_metrics_forward(const GsrMetricsArgs* args, void* stream);
+
 /* Optional per-stage device timing (cudaEvents on the caller's stream around each stage of the
  * next forward / backward calls).  The caller synchronises the stream, then reads the stage times of
  * the most recent calls in milliseconds (-1 for stages that did not run).  Not thread-safe.        */

@@ -155,6 +155,25 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan(uint32_t x) {
     return x;
 }
 
+// Deterministic block sum of N doubles per thread over a THREADS-thread block: warp shuffles, then the warps in order.
+// Result in thread 0.  sh: [THREADS / 32][N] shared doubles.
+template <int THREADS, int N>
+__device__ __forceinline__ void block_sum_f64(double (&v)[N], double (*sh)[N]) {
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) sh[warp][k] = v[k];
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < THREADS / 32; ++w)
+#pragma unroll
+            for (int k = 0; k < N; ++k) v[k] += sh[w][k];
+}
+
 // per-tile instance lists + ranges from the depth-ordered Gaussians (binning.cu)
 int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R, size_t N1, const BinScratch& bs,
                      uint32_t* point_list, uint2* ranges, cudaStream_t s, bool debug);

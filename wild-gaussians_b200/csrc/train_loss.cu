@@ -42,24 +42,6 @@ static int tl_ctas(long long HW) {
     return (int)(n < TL_MAX_CTAS ? n : TL_MAX_CTAS);
 }
 
-// Deterministic block sum of N doubles per thread: warp shuffles, then the warps in order.  Result in thread 0.
-template <int N>
-__device__ __forceinline__ void block_sum(double (&v)[N], double (*sh)[N]) {
-#pragma unroll
-    for (int k = 0; k < N; ++k)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < N; ++k) sh[warp][k] = v[k];
-    __syncthreads();
-    if (threadIdx.x == 0)
-        for (int w = 1; w < TL_THREADS / 32; ++w)
-#pragma unroll
-            for (int k = 0; k < N; ++k) v[k] += sh[w][k];
-}
-
 struct TlScratch {
     double* pix;          // [TL_MAX_CTAS][TL_PIX_SUMS]
     double* map;          // [TL_MAX_CTAS][TL_MAP_SUMS]
@@ -108,7 +90,7 @@ __global__ void __launch_bounds__(TL_THREADS) train_loss_pixels_kernel(GsrTrainL
         }
         if (a.mask) acc[5] += m;
     }
-    block_sum(acc, sh);
+    block_sum_f64<TL_THREADS>(acc, sh);
     if (threadIdx.x == 0)
 #pragma unroll
         for (int k = 0; k < TL_PIX_SUMS; ++k) s.pix[(size_t)blockIdx.x * TL_PIX_SUMS + k] = acc[k];
@@ -127,7 +109,7 @@ __global__ void __launch_bounds__(TL_THREADS) train_loss_ssim_kernel(GsrTrainLos
         acc[1] += S;
         if (a.mask) acc[2] += __fmul_rn(S, a.mask[p]);
     }
-    block_sum(acc, shm);
+    block_sum_f64<TL_THREADS>(acc, shm);
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int k = 0; k < TL_MAP_SUMS; ++k) s.map[(size_t)blockIdx.x * TL_MAP_SUMS + k] = acc[k];
@@ -147,7 +129,7 @@ __global__ void __launch_bounds__(TL_THREADS) train_loss_ssim_kernel(GsrTrainLos
     for (int b = threadIdx.x; b < (int)gridDim.x; b += TL_THREADS)
 #pragma unroll
         for (int k = 0; k < TL_MAP_SUMS; ++k) tot[TL_PIX_SUMS + k] += __ldcg(s.map + (size_t)b * TL_MAP_SUMS + k);
-    block_sum(tot, sh);
+    block_sum_f64<TL_THREADS>(tot, sh);
     if (threadIdx.x != 0) return;
     *s.ticket = 0u;
     // means, the loss and psnr from the double sums, each rounded to fp32 once

@@ -103,6 +103,12 @@ class GsrTrainLossArgs(Structure):      # include/gsrast.h
                                          "d_raw")])
 
 
+class GsrMetricsArgs(Structure):      # include/gsrast.h
+    _fields_ = ([(n, c_int) for n in ("B", "H", "W", "C", "a_u8", "b_u8")] + [("a", c_void_p), ("b", c_void_p)] +
+                [("taps", ctypes.c_double * 11), ("c1", ctypes.c_double), ("c2", ctypes.c_double)] +
+                [(n, c_void_p) for n in ("lpips_a", "lpips_b", "sums", "scratch")])
+
+
 class GsrStats(Structure):
     _fields_ = [("num_rendered", c_int), ("num_visible", c_int), ("num_tiles", c_int), ("num_coarse", c_int)]
 
@@ -207,6 +213,10 @@ def _load():
     lib.gsr_train_loss_backward.restype = c_int
     lib.gsr_unpack_u8.argtypes = [c_int, c_int] + [c_void_p] * 5
     lib.gsr_unpack_u8.restype = c_int
+    lib.gsr_metrics_scratch_bytes.argtypes = [c_int] * 4
+    lib.gsr_metrics_scratch_bytes.restype = c_size_t
+    lib.gsr_metrics_forward.argtypes = [POINTER(GsrMetricsArgs), c_void_p]
+    lib.gsr_metrics_forward.restype = c_int
     lib.gsr_profile_enable.argtypes = [c_int]
     lib.gsr_profile_enable.restype = None
     lib.gsr_profile_stage_count.restype = c_int

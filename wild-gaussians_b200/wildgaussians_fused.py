@@ -30,7 +30,9 @@ into final-size tensors, a GPU quantile without torch's 2^24-element limit, one 
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
 through ``fused_embedding``; ``enable_method(method, train=True)`` also routes ``method.train_iteration``
 (method.py:1880-2024) through ``fused_train``: the loss block and its metrics as kernels, training images staged as
-bytes in pinned memory, one metric read-back per step.
+bytes in pinned memory, one metric read-back per step.  ``enable_metrics(evaluation)`` routes the evaluation's
+``compute_metrics`` (wildgaussians/evaluation.py:331-352) through ``fused_metrics``: SSIM, MSE and MAE as kernels, LPIPS
+fed from device memory, one synchronisation per call.
 Two configurations are accelerated, which covers all three presets the reference ships: appearance on with separate
 tuned colour, ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features (the default, and the phototourism
 preset), and appearance off with SH degree 3 (the NeRF On-the-go preset; ``embedding`` is then ignored, as the
@@ -378,6 +380,51 @@ def optimize_embedding(method, dataset, *, embedding=None):
     the method's own implementation."""
     import fused_embedding
     return fused_embedding.optimize_embedding(method, dataset, embedding=embedding)
+
+
+def _metrics_hook(original, evaluation):
+    """A stand-in for evaluation.py's ``compute_metrics`` (:331-352): ``fused_metrics.compute_metrics`` where it supports
+    the input, ``original`` otherwise (no CUDA device, images under 11 pixels, other dtypes or shapes)."""
+    import fused_metrics
+
+    def compute_metrics(pred, gt, *, reduce=True, run_lpips_vgg=False):
+        if fused_metrics.supported(pred, gt):
+            return fused_metrics.compute_metrics(pred, gt, reduce=reduce, run_lpips_vgg=run_lpips_vgg, evaluation=evaluation)
+        return original(pred, gt, reduce=reduce, run_lpips_vgg=run_lpips_vgg)
+
+    compute_metrics.__wrapped__ = original
+    return compute_metrics
+
+
+def _modules_binding(evaluation, fn):
+    """The evaluation module and every loaded module whose global ``compute_metrics`` is ``fn``."""
+    mods = [evaluation] + [m for m in list(sys.modules.values()) if m is not evaluation]
+    return [m for m in mods if getattr(m, "__dict__", {}).get("compute_metrics") is fn]
+
+
+def enable_metrics(evaluation):
+    """Rebind ``compute_metrics`` of the reference's ``evaluation`` module, and of every loaded module that imported the
+    same function by name (``train.py``'s ``from .evaluation import compute_metrics``), to a hook that runs
+    ``fused_metrics.compute_metrics`` for supported input and the original otherwise.  Objects that captured the function
+    earlier keep it: ``NerfWEvaluationProtocol`` stores it in ``__init__``, so an instance built after this call takes the
+    fused path and one built before keeps the original.  ``disable_metrics`` undoes the rebinding."""
+    original = evaluation.compute_metrics
+    if hasattr(original, "__wrapped__"):
+        return evaluation
+    hook = _metrics_hook(original, evaluation)
+    for m in _modules_binding(evaluation, original):
+        m.compute_metrics = hook
+    return evaluation
+
+
+def disable_metrics(evaluation):
+    """Restore the original ``compute_metrics`` in every module ``enable_metrics`` rebound."""
+    hook = evaluation.compute_metrics
+    original = getattr(hook, "__wrapped__", None)
+    if original is not None:
+        for m in _modules_binding(evaluation, hook):
+            m.compute_metrics = original
+    return evaluation
 
 
 def enable_method(method, train: bool = False, **kw):
