@@ -191,6 +191,29 @@ int gsr_forward_recolor(const GsrForwardArgs* args, const void* geom_buffer,
                         const void* binning_buffer, const void* img_buffer,
                         void* img_buffer2, void* stream);
 
+/* Display composite of an inference render (WildGaussians.render): after gsr_forward_geometry, tile binning and one
+ * composite over the whole image that walks the tile lists with the training composite's arithmetic (the colour sums and
+ * T are its bits) but keeps no backward state (no final_T, n_contrib or blend masks in img_buffer; only the tile ranges)
+ * and writes, instead of args->out_color (which is ignored and may be NULL):
+ *   out_color [H,W,3]  clamp(C + T bg, 0, 1), then NaN -> 0 (the reference's clamp + nan_to_num_, permuted to HWC)
+ *   out_accum [H,W]    1 - T
+ *   out_depth [H,W]    with depth != 0: D + T bg[0], D composited from one value per Gaussian by the colours' recurrence
+ *                      fma(T, alpha d, D).  The values are depth_values [P] when given, otherwise the camera distance
+ *                      |means3D - campos| (in the reference's norm's operation order), computed into depth_scratch [P]
+ *                      first.
+ * Takes the arguments of gsr_forward_render otherwise.  A tile-row shard or peer images are rejected (GSR_E_INVALID).
+ * P = 0 writes nothing.                                                                                                */
+typedef struct GsrDisplayArgs {
+    float* out_color;
+    float* out_accum;
+    int    depth;
+    float* out_depth;
+    const float* depth_values;
+    float* depth_scratch;
+} GsrDisplayArgs;
+int gsr_forward_display(const GsrForwardArgs* args, const GsrDisplayArgs* display, void* geom_buffer, void* img_buffer,
+                        void* binning_buffer, void* scratch, int num_rendered, int num_coarse, void* stream);
+
 /* -- backward ---------------------------------------------------------------------------- */
 size_t gsr_backward_scratch_bytes(int P);
 int    gsr_backward(const GsrBackwardArgs* args, void* stream);

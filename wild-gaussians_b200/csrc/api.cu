@@ -434,6 +434,54 @@ int gsr_forward_recolor(const GsrForwardArgs* a, const void* geom_buffer, const 
     return 0;
 }
 
+int gsr_forward_display(const GsrForwardArgs* a, const GsrDisplayArgs* d, void* geom_buffer, void* img_buffer,
+                        void* binning_buffer, void* scratch, int num_rendered, int num_coarse, void* stream) {
+    if (!a || !d) { set_error("args / display is NULL"); return GSR_E_INVALID; }
+    GsrForwardArgs c = *a;
+    c.out_color = d->out_color;             // the display image stands in for out_color in the common checks
+    int rc = check_fwd_args(&c);
+    if (rc) return rc;
+    if (a->tile_y0 != 0 || a->tile_y1 != 0) { set_error("the display composite renders the whole image: tile-row shard set"); return GSR_E_INVALID; }
+    if (a->peer_images || a->n_peer_images) { set_error("the display composite takes no peer images"); return GSR_E_INVALID; }
+    if (num_rendered < 0 || num_coarse < 0) { set_error("bad counts"); return GSR_E_INVALID; }
+    if (a->P == 0) return 0;
+    if (!d->out_color || !d->out_accum) { set_error("out_color / out_accum is NULL"); return GSR_E_INVALID; }
+    if (d->depth && !d->out_depth) { set_error("depth requested but out_depth is NULL"); return GSR_E_INVALID; }
+    if (d->depth && !d->depth_values && (!d->depth_scratch || !a->campos)) {
+        set_error("camera distances need depth_scratch and campos");
+        return GSR_E_INVALID;
+    }
+    if (!geom_buffer || !img_buffer || (num_rendered > 0 && (!binning_buffer || !scratch))) {
+        set_error("a buffer is NULL");
+        return GSR_E_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool dbg = a->debug != 0;
+    GeomState g;
+    ImgState im;
+    BinState b;
+    BinScratch bs;
+    carve_geom((char*)geom_buffer, a->P, a->M, &g);
+    carve_img((char*)img_buffer, a->W, a->H, &im);
+    carve_bin((char*)binning_buffer, (size_t)num_rendered, &b);
+    carve_bin_scratch((char*)scratch, (size_t)num_coarse, a->W, a->H, &bs);
+    const float* depth_values = d->depth_values;
+    if (d->depth && !depth_values) {
+        rc = launch_camera_distance(a->P, a->means3D, a->campos, d->depth_scratch, s);
+        if (rc) return rc;
+        GSR_STAGE(s, dbg, "camera_distance_kernel");
+        depth_values = d->depth_scratch;
+    }
+    rc = run_tile_binning(g, a->P, a->W, a->H, (size_t)num_rendered, (size_t)num_coarse, bs, b.point_list, im.ranges, s, dbg);
+    if (rc) return rc;
+    prof_begin(ST_RENDER_FWD, s);
+    rc = launch_render_display(*a, *d, g, b, im, a->colors_precomp ? a->colors_precomp : g.rgb, depth_values, s);
+    if (rc) return rc;
+    GSR_STAGE(s, dbg, "render_fwd_packed_kernel(display)");
+    prof_end(ST_RENDER_FWD, s);
+    return 0;
+}
+
 size_t gsr_backward_scratch_bytes(int P) { return (size_t)(P > 0 ? P : 0) * sizeof(BwdAccum) + 256; }
 
 static int check_bwd_args(const GsrBackwardArgs* a, bool need_pix, bool need_outputs) {

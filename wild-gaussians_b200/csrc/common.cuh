@@ -183,6 +183,12 @@ int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinStat
 // colour-only backward composite (render_fwd.cu): adds sum T alpha dL/dpixel into a.dL_dcolor
 int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im, int ty0,
                              int ty1, cudaStream_t s);
+// display composite of an inference render (render_fwd.cu): the whole image, no backward state, the epilogue of
+// GsrDisplayArgs; depth_values [P] is composited as a fourth channel when d.depth != 0
+int launch_render_display(const GsrForwardArgs& a, const GsrDisplayArgs& d, const GeomState& g, const BinState& b,
+                          const ImgState& im, const float* colors, const float* depth_values, cudaStream_t s);
+// dist[i] = |means3D[i] - campos| with torch.norm's operation order (render_fwd.cu)
+int launch_camera_distance(int P, const float* means3D, const float* campos, float* dist, cudaStream_t s);
 
 struct BwdAccum { float4 a, b, c; };  // per-Gaussian packed partial gradients (48 B)
 // a = {dmean2D.x, dmean2D.y, |dmean2D|, dconic.x}  b = {dconic.y, dconic.w, dopacity, dcolor.r}

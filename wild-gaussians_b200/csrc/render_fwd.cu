@@ -45,6 +45,12 @@ struct RenderFwdParams {
     // peer-mapped pointers (image all-gather fused into the composite's epilogue); NULL / 0 = local out_color only
     float* const* peer_out;
     int n_peers;
+    // display epilogue (render_fwd_packed_kernel<true, *>, gsr_forward_display): colour [H,W,3] as clamp(0, 1) then NaN -> 0,
+    // accumulation 1 - T [H,W], and with DEPTH a fourth channel composited from depth_values [P] into out_depth [H,W]
+    float* disp_color;
+    float* disp_accum;
+    float* disp_depth;
+    const float* depth_values;
 };
 
 // word `word` of 8x8 block k of this CTA's tile
@@ -244,13 +250,25 @@ struct __align__(16) FwdPairRec {     // 80 bytes
     float4 bb;     // {b, b, hx, hy}: the footprint extents for the per-warp culling
 };
 
+// torch.clamp(x, 0, 1).nan_to_num_(0) of WildGaussians.render: clamp keeps a NaN, nan_to_num turns it into 0
+__device__ __forceinline__ float display_value(float x) { return isnan(x) ? 0.f : fminf(fmaxf(x, 0.f), 1.f); }
+
+// Two instantiations of one walk.  <false, false> is the training composite: colour planes, final_T, n_contrib and the
+// blend masks the backward replays.  <true, DEPTH> is the display composite of an inference render: the same walk with
+// the same pair arithmetic, culling and early-out, so its colour sums and T are the training kernel's bits, but it keeps
+// no backward state and writes the display epilogue (RenderFwdParams::disp_*).  With DEPTH it carries a fourth channel,
+// depth_values[id] composited with the colours' recurrence fma(T, alpha c, C); the values travel as {d, d} pairs in a
+// shared array of their own (8 B per staged instance next to the 80 B record).
 // (128, 9): at most 56 registers, so that 9 CTAs (36 warps) fit an SM, as the shared memory allows
+template <bool DISPLAY, bool DEPTH>
 __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_constant__ RenderFwdParams p) {
+    static_assert(DISPLAY || !DEPTH, "the depth channel is a display output");
     using PM = PixelMap<2>;
     constexpr int THREADS = 128;
     constexpr int PB = 128;               // instances per round
     __shared__ FwdPairRec s_rec[2][PB];
     __shared__ uint32_t s_blend[PixelMap<2>::WARPS][MASK_WORDS];   // blend-mask words, written out at the end
+    __shared__ float2 s_dep[2][DEPTH ? PB : 1];                    // {d, d} of the depth channel
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
@@ -287,19 +305,21 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
     const int rounds = (total + PB - 1) / PB;
 
     float2 T = make_float2(1.f, 1.f), C0 = make_float2(0.f, 0.f), C1 = C0, C2 = C0;
+    float2 Cd = C0;                       // depth channel (DEPTH only)
     uint32_t last0 = 0, last1 = 0;
     const float2 mhalf = make_float2(-0.5f, -0.5f), one = make_float2(1.f, 1.f);
 
     if (rounds > 0) {
         // raw record of the instance this thread stages next (register prefetch)
         float4 g = make_float4(0.f, 0.f, -1.f, -1.f), c = make_float4(0.f, 0.f, 0.f, 0.f);
-        float cr = 0.f, cg = 0.f, cb = 0.f;
+        float cr = 0.f, cg = 0.f, cb = 0.f, cd = 0.f;
         auto fetch = [&](uint32_t id, bool valid) {
             if (valid) {
                 const float4* src = p.rec + 2 * (size_t)id;
                 g = src[0]; c = src[1];
                 const float* col = p.colors + 3 * (size_t)id;
                 cr = col[0]; cg = col[1]; cb = col[2];
+                if constexpr (DEPTH) cd = p.depth_values[id];
             }
         };
         auto id_of = [&](int round) -> uint32_t {
@@ -322,6 +342,7 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
                 rec.rg = make_float4(cr, cr, cg, cg);
                 rec.bb = make_float4(cb, cb, g.z, g.w);
                 s_rec[buf][tid] = rec;
+                if constexpr (DEPTH) s_dep[buf][tid] = make_float2(cd, cd);
             }
             if (r + 1 < rounds) {
                 fetch(id_next, (r + 1) * PB + tid < total);
@@ -372,14 +393,17 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
                         C0 = fma2(T, mul2(alpha, make_float2(rg.x, rg.y)), C0);
                         C1 = fma2(T, mul2(alpha, make_float2(rg.z, rg.w)), C1);
                         C2 = fma2(T, mul2(alpha, make_float2(bb.x, bb.y)), C2);
+                        if constexpr (DEPTH) Cd = fma2(T, mul2(alpha, s_dep[buf][j]), Cd);
                         T = make_float2(upd0 ? test_T.x : T.x, upd1 ? test_T.y : T.y);
                         // 1-based position of this instance in the tile's list (forward.cu:349,382)
                         const uint32_t idx = round_base + (uint32_t)j + 1u;
                         last0 = upd0 ? idx : last0;
                         last1 = upd1 ? idx : last1;
                     }
-                    const int word = (int)(round_base / 32) + w;
-                    if (lane == 0 && word < MASK_WORDS) s_blend[tid >> 5][word] = blended;
+                    if constexpr (!DISPLAY) {
+                        const int word = (int)(round_base / 32) + w;
+                        if (lane == 0 && word < MASK_WORDS) s_blend[tid >> 5][word] = blended;
+                    }
                     if (!__any_sync(0xFFFFFFFFu, live0 || live1)) break;
                 }
             }
@@ -387,14 +411,30 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
     }
 
     // PixelMap<2>: warp k is 8x8 block k.  Words of batches no warp entered are copied too; they are never read.
-    __syncthreads();
-    for (int i = tid; i < MASK_BLOCKS * MASK_WORDS; i += THREADS)
-        *blend_mask_word(p, i / MASK_WORDS, i % MASK_WORDS) = s_blend[i / MASK_WORDS][i % MASK_WORDS];
+    if constexpr (!DISPLAY) {
+        __syncthreads();
+        for (int i = tid; i < MASK_BLOCKS * MASK_WORDS; i += THREADS)
+            *blend_mask_word(p, i / MASK_WORDS, i % MASK_WORDS) = s_blend[i / MASK_WORDS][i % MASK_WORDS];
+    }
 
     const size_t plane = (size_t)p.H * p.W;
     const float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
     const float r0 = C0.x + T.x * bg0, g0 = C1.x + T.x * bg1, b0 = C2.x + T.x * bg2;
     const float r1 = C0.y + T.y * bg0, g1 = C1.y + T.y * bg1, b1 = C2.y + T.y * bg2;
+    if constexpr (DISPLAY) {
+        // the depth channel's image is channel 0 of a composite of {d, d, d}, so its background term is T bg[0]
+        const float rgb[2][3] = {{r0, g0, b0}, {r1, g1, b1}};
+        const float tT[2] = {T.x, T.y}, dd[2] = {Cd.x + T.x * bg0, Cd.y + T.y * bg0};
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            if (!inside[k]) continue;
+            float* col = p.disp_color + 3 * (size_t)pix_id[k];
+            col[0] = display_value(rgb[k][0]); col[1] = display_value(rgb[k][1]); col[2] = display_value(rgb[k][2]);
+            p.disp_accum[pix_id[k]] = 1.0f - tT[k];
+            if constexpr (DEPTH) p.disp_depth[pix_id[k]] = dd[k];
+        }
+        return;
+    }
     if (inside[0]) { p.final_T[pix_id[0]] = T.x; p.n_contrib[pix_id[0]] = last0; }
     if (inside[1]) { p.final_T[pix_id[1]] = T.y; p.n_contrib[pix_id[1]] = last1; }
     if (p.n_peers > 0) {
@@ -603,11 +643,49 @@ int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinStat
         packed = e ? atoi(e) : 1;
     }
     if (packed || p.n_peers > 0) {      // the fused all-gather epilogue exists in the packed kernel only
-        render_fwd_packed_kernel<<<grid, 128, 0, s>>>(p);
+        render_fwd_packed_kernel<false, false><<<grid, 128, 0, s>>>(p);
         count_launches(1);
         return 0;
     }
     render_fwd_kernel<1><<<grid, PixelMap<1>::THREADS, 0, s>>>(p);
+    count_launches(1);
+    return 0;
+}
+
+// ---- display composite of an inference render ------------------------------------------------------------------------
+// dist[i] = |means3D[i] - campos| in the operation order of torch.norm(means3D - campos, dim=-1) on the GPU: torch reduces
+// the 3 elements with two threads (elements 0 and 2 in the first, 1 in the second) and adds the partial sums, all rounded
+// products and sums (no fma), then a correctly rounded sqrt.
+__global__ void __launch_bounds__(256) camera_distance_kernel(int P, const float* __restrict__ means3D,
+                                                              const float* __restrict__ campos, float* __restrict__ dist) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    const float dx = means3D[3 * (size_t)i] - campos[0];
+    const float dy = means3D[3 * (size_t)i + 1] - campos[1];
+    const float dz = means3D[3 * (size_t)i + 2] - campos[2];
+    dist[i] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dz, dz)), __fmul_rn(dy, dy)));
+}
+
+int launch_camera_distance(int P, const float* means3D, const float* campos, float* dist, cudaStream_t s) {
+    if (P <= 0) return 0;
+    camera_distance_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, means3D, campos, dist);
+    count_launches(1);
+    return 0;
+}
+
+int launch_render_display(const GsrForwardArgs& a, const GsrDisplayArgs& d, const GeomState& g, const BinState& b,
+                          const ImgState& im, const float* colors, const float* depth_values, cudaStream_t s) {
+    RenderFwdParams p = {};
+    p.W = a.W; p.H = a.H; p.grid_x = tiles_x(a.W); p.ty0 = 0;
+    p.ranges = im.ranges; p.point_list = b.point_list;
+    p.subpixel_offset = reinterpret_cast<const float2*>(a.subpixel_offset);
+    p.rec = g.rec; p.colors = colors; p.bg = a.background;
+    p.disp_color = d.out_color; p.disp_accum = d.out_accum; p.disp_depth = d.out_depth; p.depth_values = depth_values;
+    dim3 grid(p.grid_x, tiles_y(a.H), 1);
+    if (d.depth)
+        render_fwd_packed_kernel<true, true><<<grid, 128, 0, s>>>(p);
+    else
+        render_fwd_packed_kernel<true, false><<<grid, 128, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

@@ -109,6 +109,11 @@ class GsrMetricsArgs(Structure):      # include/gsrast.h
                 [(n, c_void_p) for n in ("lpips_a", "lpips_b", "sums", "scratch")])
 
 
+class GsrDisplayArgs(Structure):      # include/gsrast.h
+    _fields_ = [("out_color", c_void_p), ("out_accum", c_void_p), ("depth", c_int), ("out_depth", c_void_p),
+                ("depth_values", c_void_p), ("depth_scratch", c_void_p)]
+
+
 class GsrStats(Structure):
     _fields_ = [("num_rendered", c_int), ("num_visible", c_int), ("num_tiles", c_int), ("num_coarse", c_int)]
 
@@ -128,6 +133,9 @@ def _load():
     lib.gsr_forward_async.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
     lib.gsr_forward_status.argtypes = [c_void_p, c_int, c_int, c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int)]
     lib.gsr_forward_recolor.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.gsr_forward_display.argtypes = [POINTER(GsrForwardArgs), POINTER(GsrDisplayArgs), c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_int, c_int, c_void_p]
+    lib.gsr_forward_display.restype = c_int
     lib.gsr_backward_scratch_bytes.argtypes = [c_int]
     lib.gsr_backward_scratch_bytes.restype = c_size_t
     lib.gsr_backward.argtypes = [POINTER(GsrBackwardArgs), c_void_p]

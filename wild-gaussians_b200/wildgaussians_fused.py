@@ -32,7 +32,9 @@ through ``fused_embedding``; ``enable_method(method, train=True)`` also routes `
 (method.py:1880-2024) through ``fused_train``: the loss block and its metrics as kernels, training images staged as
 bytes in pinned memory, one metric read-back per step.  ``enable_metrics(evaluation)`` routes the evaluation's
 ``compute_metrics`` (wildgaussians/evaluation.py:331-352) through ``fused_metrics``: SSIM, MSE and MAE as kernels, LPIPS
-fed from device memory, one synchronisation per call.
+fed from device memory, one synchronisation per call.  ``enable_method(method, render=True)`` routes ``method.render``
+(method.py:1832-1866) through ``fused_render``: toned colours only, one display composite that writes the clamped HWC
+colour, the accumulation and the depth, one pinned device-to-host copy.
 Two configurations are accelerated, which covers all three presets the reference ships: appearance on with separate
 tuned colour, ``appearance_model_sh`` off, SH degree 3, 24 + 32 embedding features (the default, and the phototourism
 preset), and appearance off with SH degree 3 (the NeRF On-the-go preset; ``embedding`` is then ignored, as the
@@ -427,22 +429,34 @@ def disable_metrics(evaluation):
     return evaluation
 
 
-def enable_method(method, train: bool = False, **kw):
+def render(method, camera, options=None, **kwargs):
+    """``WildGaussians.render`` on one colour pass, one geometry pass and one display composite (``fused_render``);
+    unsupported calls run the method's own implementation."""
+    import fused_render
+    return fused_render.render(method, camera, options, **kwargs)
+
+
+def enable_method(method, train: bool = False, render: bool = False, **kw):
     """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
     ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged.  With
     ``train``, ``method.train_iteration`` is rebound (instance attribute) to ``fused_train.train_iteration``: its loss
     always runs as the fused op, while the backbone, ``msssim``, the uncertainty head and densification (``densify``)
-    follow their own flags."""
+    follow their own flags.  With ``render``, ``method.render`` (every evaluation image, video frame and viewer frame) is
+    rebound (instance attribute) to ``fused_render.render``: one colour pass, one display composite and one
+    device-to-host copy into pinned memory, the same result arrays."""
     enable(method.model, **kw)
     method.optimize_embedding = types.MethodType(optimize_embedding, method)
     if train:
         import fused_train
         method.train_iteration = types.MethodType(fused_train.train_iteration, method)
+    if render:
+        method.render = types.MethodType(globals()["render"], method)
     return method
 
 
 def disable_method(method):
     method.__dict__.pop("optimize_embedding", None)
     method.__dict__.pop("train_iteration", None)
+    method.__dict__.pop("render", None)
     disable(method.model)
     return method
