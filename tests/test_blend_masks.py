@@ -6,12 +6,7 @@ pixel of the block blended that position; the backward walks only those position
   whose alpha or power lies within a hair of a threshold are not compared).
 * A scene dense enough that tile lists run past K (the footprint-box fallback of the backward) has gradients within
   the parity bar against the compiled reference.
-* GSR_FWD_PACKED=0 / GSR_BWD_PACKED=0 (read once per process, hence subprocesses) give the same masks and results.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -147,42 +142,3 @@ def test_fallback_beyond_k_against_compiled_reference():
         if a.numel() == 0:
             continue
         check_grad(n, torch.from_numpy(o["grad_" + n]).view_as(a.cpu()), a.cpu(), b.cpu())
-
-
-def _dump(path, fwd_packed, bwd_packed):
-    os.environ["GSR_FWD_PACKED"], os.environ["GSR_BWD_PACKED"] = str(fwd_packed), str(bwd_packed)
-    outs = {}
-    for i, (kw, op) in enumerate([(SMALL[1], None), (DENSE, DENSE_OPACITY)]):
-        for key, val in _run(kw, op).items():
-            outs[f"{i}_{key}"] = val
-    np.savez(path, **outs)
-
-
-@pytest.mark.parametrize("fwd_packed,bwd_packed", [(0, 1), (1, 0), (0, 0)])
-def test_scalar_kernels_give_the_same_masks_and_results(tmp_path, fwd_packed, bwd_packed):
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([here, os.path.join(here, "golden"), root,
-                                                         os.path.join(root, "wild-gaussians_b200")]))
-    files = {}
-    for fp, bp in [(1, 1), (fwd_packed, bwd_packed)]:
-        files[fp, bp] = str(tmp_path / f"f{fp}b{bp}.npz")
-        code = f"import test_blend_masks as t; t._dump({files[fp, bp]!r}, {fp}, {bp})"
-        subprocess.run([sys.executable, "-c", code], check=True, env=env, cwd=here)
-    a, b = np.load(files[1, 1]), np.load(files[fwd_packed, bwd_packed])
-    for i in range(2):
-        oa = {k[2:]: a[k] for k in a.files if k.startswith(f"{i}_")}
-        ob = {k[2:]: b[k] for k in b.files if k.startswith(f"{i}_")}
-        for k in ("color", "n_contrib", "radii", "point_list", "ranges"):
-            assert np.array_equal(oa[k], ob[k]), (i, k)
-        # mask words are defined below the block's largest n_contrib
-        valid = np.arange(K)[None, None, :] < np.minimum(_block_last(oa), K)[..., None]
-        assert np.array_equal(_unpack(oa["masks"])[valid], _unpack(ob["masks"])[valid]), i
-        if fwd_packed == 0:
-            _check_masks({**ob, "W": int(ob["W"]), "H": int(ob["H"])})
-        for n in GRAD_NAMES:
-            ga, gb = oa["grad_" + n].astype(np.float64), ob["grad_" + n].astype(np.float64)
-            if ga.size == 0:
-                continue
-            scale = np.abs(ga).max() + 1e-30
-            assert np.abs(ga - gb).max() / scale < 1e-5, (i, n)

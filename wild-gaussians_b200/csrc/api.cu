@@ -295,7 +295,7 @@ static int binning_and_render(const GsrForwardArgs* a, const GeomState& g, const
     prof_begin(ST_RENDER_FWD, s);
     rc = launch_render_fwd(*a, g, b, im, colors, ty0, ty1, s);
     if (rc) return rc;
-    GSR_STAGE(s, dbg, "render_fwd_kernel");
+    GSR_STAGE(s, dbg, "render_fwd_packed_kernel");
     prof_end(ST_RENDER_FWD, s);
     return 0;
 }
@@ -429,7 +429,7 @@ int gsr_forward_recolor(const GsrForwardArgs* a, const void* geom_buffer, const 
     prof_begin(ST_RENDER_FWD, s);
     rc = launch_render_fwd(*a, g, b, im2, a->colors_precomp, ty0, ty1, s);
     if (rc) return rc;
-    GSR_STAGE(s, a->debug != 0, "render_fwd_kernel(recolor)");
+    GSR_STAGE(s, a->debug != 0, "render_fwd_packed_kernel(recolor)");
     prof_end(ST_RENDER_FWD, s);
     return 0;
 }
@@ -533,7 +533,7 @@ static int backward_partials_impl(const GsrBackwardArgs* a, void* stream, const 
         prof_begin(ST_RENDER_BWD, s);
         rc = launch_render_bwd(*a, g, b, im, colors, accum, ty0, ty1, s, peer, touched);
         if (rc) return rc;
-        GSR_STAGE(s, dbg, "render_bwd_kernel");
+        GSR_STAGE(s, dbg, "render_bwd_packed_kernel");
         prof_end(ST_RENDER_BWD, s);
     }
     return 0;
@@ -596,11 +596,10 @@ int gsr_backward_finalize(const GsrBackwardArgs* a, void* stream) {
     if (rc) return rc;
     GSR_STAGE(s, a->debug != 0, "preprocess_bwd_kernel");
     prof_end(ST_PREPROCESS_BWD, s);
-    // leave the accumulator zeroed for the next backward pass: a caller that keeps the buffer passes accum_is_zero = 1 next
-    // time, and the tile-row sharded path needs no fill + barrier in front of its peer reductions.  The kernel clears the
-    // rows it found non-zero itself (only the Gaussians some pixel blended: 10-20 % of a dense scene; clearing ALL rows in
-    // the kernel was measured 3.5x slower than the kernel + a memset); GSR_ACCUM_CLEAR=0 keeps the stream-ordered memset.
-    if (!preprocess_bwd_clears_accum()) GSR_CUDA(cudaMemsetAsync(accum_of(a), 0, (size_t)a->P * sizeof(BwdAccum), s));
+    // the kernel left the accumulator zeroed for the next backward pass: a caller that keeps the buffer passes
+    // accum_is_zero = 1 next time, and the tile-row sharded path needs no fill + barrier in front of its peer reductions.
+    // It clears only the rows it found non-zero (the Gaussians some pixel blended: 10-20 % of a dense scene; clearing ALL
+    // rows in the kernel was measured 3.5x slower than the kernel + a memset).
     return 0;
 }
 

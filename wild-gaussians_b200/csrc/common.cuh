@@ -212,7 +212,6 @@ struct PullPeers {
 };
 int launch_preprocess_bwd(const GsrBackwardArgs& a, const GeomState& g, BwdAccum* accum, cudaStream_t s,
                           const PullPeers* pull = nullptr);
-bool preprocess_bwd_clears_accum();   // GSR_ACCUM_CLEAR (default 1): the chain-rule kernel zeroes the rows it consumed
 
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t s);
 

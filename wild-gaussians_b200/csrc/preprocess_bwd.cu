@@ -13,7 +13,6 @@
 #include "common.cuh"
 #include "gaussian_math.cuh"
 #include "sh_math.cuh"
-#include <cstdlib>
 
 namespace gsr {
 
@@ -33,7 +32,7 @@ struct PreBwdParams {
     const float* campos;
     const float4* rec;
     const float* accum;     // [P][12]
-    float* accum_clear;     // the same array when the kernel is to zero the rows it consumed (see launch_preprocess_bwd), else NULL
+    float* accum_clear;     // the same array, whose consumed rows the kernel zeroes; NULL in pull mode (the other ranks still read it)
     // pull-mode multi-GPU reduction (gsrast.h, gsr_backward_finalize_pull): complete sums = rows of all ranks in rank order
     const float* pull_accums[GSR_MAX_PULL_PEERS];            // the ranks' accumulators (peer-mapped), by value: no pointer-table load
     const unsigned char* pull_touched[GSR_MAX_PULL_PEERS];   // the ranks' mark arrays
@@ -372,16 +371,6 @@ __global__ void __launch_bounds__(256, MIN_CTAS) preprocess_bwd_kernel(const __g
     if (p.dL_drot) reinterpret_cast<float4*>(p.dL_drot)[i] = make_float4(o_rot[0], o_rot[1], o_rot[2], o_rot[3]);
 }
 
-// 1: the kernel zeroes the accumulator rows it consumed (the caller then skips its memset)
-bool preprocess_bwd_clears_accum() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("GSR_ACCUM_CLEAR");
-        v = e ? atoi(e) : 1;
-    }
-    return v != 0;
-}
-
 int launch_preprocess_bwd(const GsrBackwardArgs& a, const GeomState& g, BwdAccum* accum, cudaStream_t s, const PullPeers* pull) {
     PreBwdParams p;
     p.P = a.P; p.D = a.D; p.M = a.M;
@@ -393,7 +382,7 @@ int launch_preprocess_bwd(const GsrBackwardArgs& a, const GeomState& g, BwdAccum
     p.scales = a.scales; p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp;
     p.view = a.viewmatrix; p.proj = a.projmatrix; p.campos = a.campos;
     p.rec = g.rec; p.accum = reinterpret_cast<const float*>(accum);
-    p.accum_clear = (preprocess_bwd_clears_accum() && !pull) ? reinterpret_cast<float*>(accum) : nullptr;
+    p.accum_clear = pull ? nullptr : reinterpret_cast<float*>(accum);
     for (int r = 0; r < GSR_MAX_PULL_PEERS; ++r) {
         p.pull_accums[r] = (pull && r < pull->n_peers) ? pull->accums[r] : nullptr;
         p.pull_touched[r] = (pull && r < pull->n_peers) ? pull->touched[r] : nullptr;

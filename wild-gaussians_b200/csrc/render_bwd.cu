@@ -23,7 +23,6 @@
 // The |grad| channel (backward.cu:593-595) is the sum over pixels of |gx| + |gy|, so the
 // absolute value is taken per lane BEFORE the warp reduction.
 #include "render_common.cuh"
-#include <cstdlib>
 
 namespace gsr {
 
@@ -186,219 +185,11 @@ __device__ __forceinline__ float rcp_approx(float x) {
     return r;
 }
 
-// What one lane accumulates per Gaussian (summed over its pixels, then over the warp, then over the tile).
-// With w = G * dL/dalpha of a blended (pixel, Gaussian) pair and d = mean2D - pixel:
-//   0: sum w*dx   1: sum w*dy   2: sum |dL/dmean2D.x| + |dL/dmean2D.y|   3: sum w*dx*dx   4: sum w*dx*dy
-//   5: sum w*dy*dy   6: sum w (= dL/d(opacity*coef))   7..9: sum alpha*T*dL/dpixel[ch] (= dL/dcolour)
-// The reference's per-pair gradient terms (backward.cu:574-603) are linear in these moments:
-//   dL/dmean2D.x = -o W/2 (A s0 + B s1)   dL/dmean2D.y = -o H/2 (C s1 + B s0)   dL/dconic = -o/2 (s3, s4, s5)
-// (o = opacity*coef, (A, B, C) = conic), so the linear map is applied once per (tile, Gaussian) when the tile
-// flushes its sums instead of once per pixel pair.
-template <int PPT>
-__global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_bwd_kernel(const __grid_constant__ RenderBwdParams p) {
-    using PM = PixelMap<PPT>;
-    constexpr int THREADS = PM::THREADS;
-    constexpr int WARPS = PM::WARPS;
-    constexpr int RB = 64;   // instances staged per round: four private rows of 64 slots keep the shared memory small
-    static_assert(RB <= THREADS, "one staged instance per thread");
-    __shared__ uint32_t s_id[RB];
-    __shared__ __align__(16) float4 s_geo[RB];   // {x, y, hx, hy}
-    __shared__ __align__(16) float4 s_con[RB];   // {conic.x, conic.y, conic.z, opacity}
-    __shared__ __align__(16) float4 s_col[RB];   // {r, g, b, -}
-    __shared__ PartRows<WARPS, RB> s_part;
-    __shared__ uint32_t s_max[WARPS];
-    constexpr int NW = RB / 32 + 1;   // mask words a round's positions can span
-    __shared__ uint32_t s_mask[WARPS][NW];
-    static_assert(WARPS == MASK_BLOCKS, "one warp per 8x8 blend-mask block");
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
-    const size_t plane = (size_t)p.H * p.W;
-    const float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
-
-    // per-pixel state.  Tb = -T_final * (bg . dL/dpixel): the background term of dL/dalpha is Tb / (1 - alpha)
-    // (backward.cu:576-579).  rdot / last_cd / last_alpha carry the reference's accum_rec / last_color / last_alpha
-    // recurrence (backward.cu:560-572) projected on dL/dpixel: only (colour - accum_rec) . dL/dpixel is ever used.
-    float2 pixf[PPT];
-    float T[PPT], Tb[PPT], rdot[PPT], last_cd[PPT], last_alpha[PPT];
-    uint32_t last_contributor[PPT];
-    float dL_dpixel[PPT][3];
-    float bx0 = 3.0e38f, bx1 = -3.0e38f, by0 = 3.0e38f, by1 = -3.0e38f;
-    uint32_t thread_last = 0;
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        int lx, ly;
-        PM::pixel(tid, k, lx, ly);
-        const unsigned px = tile_x * TILE + lx, py = tile_y * TILE + ly;
-        const unsigned pix_id = p.W * py + px;
-        const bool inside = px < (unsigned)p.W && py < (unsigned)p.H;
-        pixf[k] = {(float)px, (float)py};
-        T[k] = 0.f;
-        last_contributor[k] = 0;
-#pragma unroll
-        for (int ch = 0; ch < 3; ++ch) dL_dpixel[k][ch] = 0.f;
-        if (inside) {
-            const float2 so = p.subpixel_offset[pix_id];
-            pixf[k].x += so.x;
-            pixf[k].y += so.y;
-            T[k] = p.final_T[pix_id];
-            last_contributor[k] = p.n_contrib[pix_id];
-#pragma unroll
-            for (int ch = 0; ch < 3; ++ch) dL_dpixel[k][ch] = p.dL_dpix[ch * plane + pix_id];
-            bx0 = fminf(bx0, pixf[k].x); bx1 = fmaxf(bx1, pixf[k].x);
-            by0 = fminf(by0, pixf[k].y); by1 = fmaxf(by1, pixf[k].y);
-        }
-        Tb[k] = -T[k] * (bg0 * dL_dpixel[k][0] + bg1 * dL_dpixel[k][1] + bg2 * dL_dpixel[k][2]);
-        rdot[k] = 0.f; last_cd[k] = 0.f; last_alpha[k] = 0.f;
-        thread_last = max(thread_last, last_contributor[k]);
-    }
-    const WarpBox box = warp_box_reduce(bx0, bx1, by0, by1);
-    const uint2 range = p.ranges[tile_y * p.grid_x + tile_x];
-
-    // warp-wide and tile-wide largest last_contributor: nothing behind it contributes
-    const uint32_t warp_last = __reduce_max_sync(0xFFFFFFFFu, thread_last);
-    if (lane == 0) s_max[warp] = warp_last;
-    __syncthreads();
-    uint32_t tile_last = 0;
-#pragma unroll
-    for (int w = 0; w < WARPS; ++w) tile_last = max(tile_last, s_max[w]);
-    const int total = (int)min(tile_last, range.y - range.x);   // instances [range.x, range.x+total) matter
-    const int rounds = (total + RB - 1) / RB;
-
-    // Gradient of pixel coordinate w.r.t. normalized screen-space viewport coordinates (-1 to 1)
-    const float ddelx_dx = 0.5f * p.W;
-    const float ddely_dy = 0.5f * p.H;
-
-    // which butterfly slot this lane ends up holding is a function of the lane only
-    int my_slot;
-    {
-        float dummy[10];
-#pragma unroll
-        for (int q = 0; q < 10; ++q) dummy[q] = 0.f;
-        my_slot = butterfly10(dummy, lane);
-    }
-    const bool slot_owner = (lane & 1) == 0 && my_slot < 10;
-
-    int toDo = total;
-    for (int r = 0; r < rounds; ++r, toDo -= RB) {
-        const int n = min(RB, toDo);
-        // 0-based list position of staged entry j: pos(j) = first_pos - j  (walking back to front)
-        const int first_pos = total - 1 - r * RB;
-        const int w_lo = (first_pos - n + 1) >> 5;
-        __syncthreads();   // previous round's rows flushed, staging buffers free
-        stage_mask_words<WARPS, NW>(p, tile_y * p.grid_x + tile_x, w_lo, s_max, s_mask);
-        if (tid < n) {
-            const uint32_t id = p.point_list[range.x + first_pos - tid];
-            s_id[tid] = id;
-            const float4* src = p.rec + 2 * (size_t)id;
-            s_geo[tid] = src[0];
-            s_con[tid] = src[1];
-            const float* c = p.colors + 3 * (size_t)id;
-            s_col[tid] = make_float4(c[0], c[1], c[2], 0.f);
-        }
-        __syncthreads();
-
-#pragma unroll 1
-        for (int w = 0; w < RB / 32; ++w) {
-            // per-warp culling: the positions the forward blended in this warp's block (bwd_walks)
-            const int jl = w * 32 + lane;
-            const bool rel = jl < n && bwd_walks(first_pos - jl, warp_last, w_lo, s_mask[warp], s_geo[jl], s_con[jl], box);
-            unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
-            uint32_t wrote = 0;
-            while (mm) {
-                const int j = w * 32 + __ffs(mm) - 1;
-                mm &= mm - 1;
-                const uint32_t pos = (uint32_t)(first_pos - j);
-                const float4 geo = s_geo[j];
-                const float4 con_o = s_con[j];
-
-                // pass 1: which of this lane's pixels blend this Gaussian (same tests, same expressions as the
-                // forward: backward.cu:529-546 / forward.cu:353-368)
-                float G[PPT], alpha[PPT];
-                float2 d[PPT];
-                bool any_active = false;
-#pragma unroll
-                for (int k = 0; k < PPT; ++k) {
-                    d[k] = {geo.x - pixf[k].x, geo.y - pixf[k].y};
-                    const float power = -0.5f * (con_o.x * d[k].x * d[k].x + con_o.z * d[k].y * d[k].y) - con_o.y * d[k].x * d[k].y;
-                    const float g = expf(power);
-                    const float a = min(0.99f, con_o.w * g);
-                    // the reference visits an instance iff its position is below the pixel's n_contrib
-                    // (backward.cu:529-533); pixels outside the image have n_contrib = 0
-                    const bool act = pos < last_contributor[k] && !(power > 0.0f) && !(a < 1.0f / 255.0f);
-                    // a pair that does not blend is carried through the arithmetic below as G = alpha = 0: T, the
-                    // sums and the recurrence are then unchanged (the pending accum_rec update is merely applied
-                    // one step early, which commutes)
-                    G[k] = act ? g : 0.f;
-                    alpha[k] = act ? a : 0.f;
-                    any_active |= act;
-                }
-                // below MASK_K some pixel of the warp blends by construction; above, the box test is only conservative
-                if (pos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, any_active)) continue;   // warp-uniform
-
-                const float4 col = s_col[j];
-                const float kx = fabsf(con_o.w) * ddelx_dx, ky = fabsf(con_o.w) * ddely_dy;
-                float v[10];
-#pragma unroll
-                for (int k = 0; k < PPT; ++k) {
-                    // T before this splat; 1 - alpha is in [0.01, 1], the approximate reciprocal is good to 1 ulp
-                    // and gradients are compared at 1e-3 (backward.cu:548,579 divide twice)
-                    const float inv = rcp_approx(1.f - alpha[k]);
-                    T[k] *= inv;
-                    const float aT = alpha[k] * T[k];
-                    rdot[k] = fmaf(last_alpha[k], last_cd[k] - rdot[k], rdot[k]);
-                    const float cd = col.x * dL_dpixel[k][0] + col.y * dL_dpixel[k][1] + col.z * dL_dpixel[k][2];
-                    last_cd[k] = cd;
-                    last_alpha[k] = alpha[k];
-                    const float dL_dalpha = fmaf(cd - rdot[k], T[k], Tb[k] * inv);
-                    const float wgt = G[k] * dL_dalpha;
-                    const float wx = wgt * d[k].x, wy = wgt * d[k].y;
-                    const float t1 = con_o.x * wx + con_o.y * wy;
-                    const float t2 = con_o.z * wy + con_o.y * wx;
-                    const float ab = fmaf(fabsf(t2), ky, fabsf(t1) * kx);
-                    if (k == 0) {
-                        v[0] = wx; v[1] = wy; v[2] = ab;
-                        v[3] = wx * d[k].x; v[4] = wx * d[k].y; v[5] = wy * d[k].y;
-                        v[6] = wgt;
-                        v[7] = aT * dL_dpixel[k][0]; v[8] = aT * dL_dpixel[k][1]; v[9] = aT * dL_dpixel[k][2];
-                    } else {
-                        v[0] += wx; v[1] += wy; v[2] += ab;
-                        v[3] = fmaf(wx, d[k].x, v[3]); v[4] = fmaf(wx, d[k].y, v[4]); v[5] = fmaf(wy, d[k].y, v[5]);
-                        v[6] += wgt;
-                        v[7] = fmaf(aT, dL_dpixel[k][0], v[7]); v[8] = fmaf(aT, dL_dpixel[k][1], v[8]);
-                        v[9] = fmaf(aT, dL_dpixel[k][2], v[9]);
-                    }
-                }
-                butterfly10(v, lane);
-                if (slot_owner) reinterpret_cast<float*>(s_part.row[warp][j])[my_slot] = v[0];
-                wrote |= 1u << (j - w * 32);
-            }
-            if (lane == 0) s_part.wrote[warp][w] = wrote;
-        }
-        __syncthreads();
-        // one flush per visited Gaussian per tile: moments -> gradient terms, three 128-bit reductions
-        // (skipped when nothing landed)
-        float4 a0, a1, a2;
-        if (tid < n && s_part.sum(tid, a0, a1, a2)) {
-            const bool any = (a0.x != 0.f) | (a0.y != 0.f) | (a0.z != 0.f) | (a0.w != 0.f) | (a1.x != 0.f) |
-                             (a1.y != 0.f) | (a1.z != 0.f) | (a1.w != 0.f) | (a2.x != 0.f) | (a2.y != 0.f);
-            if (any) {
-                const float4 con_o = s_con[tid];
-                const float o = con_o.w;
-                const float gx = -o * ddelx_dx * (con_o.x * a0.x + con_o.y * a0.y);
-                const float gy = -o * ddely_dy * (con_o.z * a0.y + con_o.y * a0.x);
-                const float h = -0.5f * o;
-                flush_row<false>(p, s_id[tid], make_float4(gx, gy, a0.z, h * a0.w), make_float4(h * a1.x, h * a1.y, a1.z, a1.w),
-                          make_float4(a2.x, a2.y, 0.f, 0.f));
-            }
-        }
-    }
-}
-
-// ---- packed variant: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2, render_common.cuh) ----
-// Both pixels of a lane share every per-Gaussian operand load and the loop control, and the fused epilogues (peer
-// reduction, touched marks) exist in this kernel only.  IEEE rounding per element is that of the scalar instruction: the expression shapes that decide which pairs blend
-// (power, alpha; forward.cu:353-368) are the same trees as in the scalar kernel, fused exactly where nvcc fuses them.
+// ---- packed composite: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2, render_common.cuh) ----
+// Both pixels of a lane share every per-Gaussian operand load and the loop control.  Every element is rounded as the
+// scalar instruction, and the expressions that decide which pairs blend (power, alpha; forward.cu:353-368) are the
+// forward's, fused exactly where nvcc fuses the reference's scalar expressions, so a pixel blends the positions it
+// blended in the forward.
 // Per-Gaussian operands are staged in shared memory already duplicated ({x, x, y, y} ...) so that one LDS.128 yields
 // two ready-made broadcast pairs and no register moves are needed.
 struct __align__(16) PairRec {      // 80 bytes per staged Gaussian
@@ -412,10 +203,18 @@ struct __align__(16) PairRec {      // 80 bytes per staged Gaussian
 __device__ __forceinline__ float2 lo2(const float4 v) { return make_float2(v.x, v.y); }
 __device__ __forceinline__ float2 hi2(const float4 v) { return make_float2(v.z, v.w); }
 
+// What one lane accumulates per Gaussian (summed over its pixels, then over the warp, then over the tile).
+// With w = G * dL/dalpha of a blended (pixel, Gaussian) pair and d = mean2D - pixel:
+//   0: sum w*dx   1: sum w*dy   2: sum |dL/dmean2D.x| + |dL/dmean2D.y|   3: sum w*dx*dx   4: sum w*dx*dy
+//   5: sum w*dy*dy   6: sum w (= dL/d(opacity*coef))   7..9: sum alpha*T*dL/dpixel[ch] (= dL/dcolour)
+// The reference's per-pair gradient terms (backward.cu:574-603) are linear in these moments:
+//   dL/dmean2D.x = -o W/2 (A s0 + B s1)   dL/dmean2D.y = -o H/2 (C s1 + B s0)   dL/dconic = -o/2 (s3, s4, s5)
+// (o = opacity*coef, (A, B, C) = conic), so the linear map is applied once per (tile, Gaussian) when the tile
+// flushes its sums instead of once per pixel pair.
 // (128, 9): at most 56 registers, so that 9 CTAs (36 warps) fit an SM, as the shared memory allows
 template <bool PEER>
 __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_constant__ RenderBwdParams p) {
-    using PM = PixelMap<2>;
+    using PM = PixelMap;
     constexpr int THREADS = PM::THREADS;   // 128
     constexpr int WARPS = PM::WARPS;       // 4
     constexpr int PB = 64;                 // instances staged per round: four private rows of 64 slots keep 9 CTAs/SM
@@ -432,7 +231,10 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
     const size_t plane = (size_t)p.H * p.W;
     const float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
 
-    // per-pixel state, pixel 0 in .x and pixel 1 in .y of every pair
+    // per-pixel state, pixel 0 in .x and pixel 1 in .y of every pair.  Tb = -T_final * (bg . dL/dpixel): the background
+    // term of dL/dalpha is Tb / (1 - alpha) (backward.cu:576-579).  rdot / last_cd / last_alpha carry the reference's
+    // accum_rec / last_color / last_alpha recurrence (backward.cu:560-572) projected on dL/dpixel: only
+    // (colour - accum_rec) . dL/dpixel is ever used.
     float2 npx, npy, T, Tb, rdot, last_cd, last_alpha, dL0, dL1, dL2;
     uint32_t last_contributor[2];
     float bx0 = 3.0e38f, bx1 = -3.0e38f, by0 = 3.0e38f, by1 = -3.0e38f;
@@ -467,6 +269,7 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
     const WarpBox box = warp_box_reduce(bx0, bx1, by0, by1);
     const uint2 range = p.ranges[tile_y * p.grid_x + tile_x];
 
+    // warp-wide and tile-wide largest last_contributor: nothing behind it contributes
     const uint32_t warp_last = __reduce_max_sync(0xFFFFFFFFu, max(last_contributor[0], last_contributor[1]));
     if (lane == 0) s_max[warp] = warp_last;
     __syncthreads();
@@ -479,6 +282,7 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
     const float2 mhalf = make_float2(-0.5f, -0.5f), one = make_float2(1.f, 1.f);
 
+    // which butterfly slot this lane ends up holding is a function of the lane only
     int my_slot;
     {
         float dummy[10];
@@ -491,6 +295,7 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
     int toDo = total;
     for (int r = 0; r < rounds; ++r, toDo -= PB) {
         const int n = min(PB, toDo);
+        // 0-based list position of staged entry j: pos(j) = first_pos - j  (walking back to front)
         const int first_pos = total - 1 - r * PB;
         const int w_lo = (first_pos - n + 1) >> 5;
         __syncthreads();
@@ -539,15 +344,22 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
                 const float g0 = expf(power.x), g1 = expf(power.y);
                 const float2 oG = mul2(hi2(bo), make_float2(g0, g1));
                 const float a0 = min(0.99f, oG.x), a1 = min(0.99f, oG.y);
+                // the reference visits an instance iff its position is below the pixel's n_contrib (backward.cu:529-533);
+                // pixels outside the image have n_contrib = 0
                 const bool act0 = pos < last_contributor[0] && !(power.x > 0.0f) && !(a0 < 1.0f / 255.0f);
                 const bool act1 = pos < last_contributor[1] && !(power.y > 0.0f) && !(a1 < 1.0f / 255.0f);
-                if (pos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, act0 || act1)) continue;   // see the scalar kernel
-                // pairs that do not blend run through the arithmetic as G = alpha = 0 (see the scalar kernel)
+                // below MASK_K some pixel of the warp blends by construction; above, the box test is only conservative
+                if (pos >= (uint32_t)MASK_K && !__any_sync(0xFFFFFFFFu, act0 || act1)) continue;   // warp-uniform
+                // a pair that does not blend is carried through the arithmetic below as G = alpha = 0: T, the sums and
+                // the recurrence are then unchanged (the pending accum_rec update is merely applied one step early,
+                // which commutes)
                 const float2 G = make_float2(act0 ? g0 : 0.f, act1 ? g1 : 0.f);
                 const float2 alpha = make_float2(act0 ? a0 : 0.f, act1 ? a1 : 0.f);
 
                 const float4 rg = R.rg, bk = R.bk;
                 const float2 oma = add2(one, make_float2(-alpha.x, -alpha.y));
+                // T before this splat; 1 - alpha is in [0.01, 1], the approximate reciprocal is good to 1 ulp and gradients
+                // are compared at 1e-3 (backward.cu:548,579 divide twice)
                 const float2 inv = make_float2(rcp_approx(oma.x), rcp_approx(oma.y));
                 T = mul2(T, inv);
                 const float2 aT = mul2(alpha, T);
@@ -616,22 +428,10 @@ int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinSta
     p.accum = reinterpret_cast<float*>(accum);
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);
-    static int packed = -1;
-    if (packed < 0) {
-        const char* e = getenv("GSR_BWD_PACKED");     // tuning aid: 1 = 2 pixels/lane in paired fp32 instructions
-        packed = e ? atoi(e) : 1;
-    }
-    if (peer) {   // the reduction-fused flush exists in the packed kernel only
+    if (peer)   // the flush adds into every rank's accumulator
         render_bwd_packed_kernel<true><<<grid, 128, 0, s>>>(p);
-        count_launches(1);
-        return 0;
-    }
-    if (packed || touched) {    // the marks are written by the packed kernel's flush only
+    else
         render_bwd_packed_kernel<false><<<grid, 128, 0, s>>>(p);
-        count_launches(1);
-        return 0;
-    }
-    render_bwd_kernel<2><<<grid, PixelMap<2>::THREADS, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

@@ -4,24 +4,9 @@
 
 namespace gsr {
 
-constexpr int RT_BATCH = 256;   // instances staged in shared memory per round
-
-__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gmem_src) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async_4(void* smem_dst, const void* gmem_src) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(d), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
-}
-
 // Pair arithmetic of the packed composite kernels: each element is rounded exactly like the scalar instruction and
-// never contracted, so a pair gives the scalar kernel's bits.  sm_90 has no 2-wide fp32 instructions; the pairing
+// never contracted, so a kernel that spells out the reference's expressions with these (fma2 exactly where nvcc fuses
+// the reference's scalar expressions) gives the reference's bits.  sm_90 has no 2-wide fp32 instructions; the pairing
 // keeps the packed kernels' staging (one LDS.128 = two ready-made broadcast pairs) and their fused epilogues.
 __device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
@@ -29,14 +14,13 @@ __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
     return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
-// Thread -> pixel mapping inside a 16x16 tile.  A thread owns PPT vertically adjacent pixels (1 or 2), a warp owns a
-// compact block of 8 x (4 PPT) pixels (the reference: one pixel per thread, a warp = a 16x2 strip).  Per-pixel
-// results do not depend on the mapping.  Two pixels per thread amortise the per-Gaussian shared-memory loads, loop
-// control and (in the backward) the warp reduction over more (pixel, Gaussian) pairs; the compact block keeps the
-// per-warp culling selective and every 32-byte output sector is written by one warp.
-template <int PPT>
+// Thread -> pixel mapping inside a 16x16 tile.  A thread owns 2 vertically adjacent pixels (k = 0, 1), a warp owns a
+// compact 8x8 block, warp k being block k of the blend masks (the reference: one pixel per thread, a warp = a 16x2
+// strip).  Per-pixel results do not depend on the mapping.  Two pixels per thread amortise the per-Gaussian
+// shared-memory loads, loop control and (in the backward) the warp reduction over more (pixel, Gaussian) pairs; the
+// compact block keeps the per-warp culling selective and every 32-byte output sector is written by one warp.
 struct PixelMap {
-    static_assert(PPT == 1 || PPT == 2, "PPT must be 1 or 2");
+    static constexpr int PPT = 2;                       // pixels per thread
     static constexpr int THREADS = TILE * TILE / PPT;
     static constexpr int WARPS = THREADS / 32;
     static constexpr int BW = 8, BH = 4 * PPT;          // warp block in pixels

@@ -1,31 +1,32 @@
 // render_fwd.cu -- per-tile front-to-back alpha compositing.
 // Replaces renderCUDA<3> of the reference (forward.cu:273-395).
 //
-// One CTA per 16x16 tile; a thread owns PPT pixels, a warp a compact pixel block (render_common.cuh).
-// The tile's slice of the sorted instance list is consumed in rounds of 256 instances; each round's
-// 32-byte projected records and colours are gathered into shared memory with asynchronous copies
-// (cp.async / LDGSTS, no register staging) into a double buffer, two rounds of Gaussian ids ahead, so
-// the gather of round r+1 overlaps the blending of round r.  Colours are staged too (the reference
-// fetches them from global memory inside the blend loop, forward.cu:376).
+// One CTA of 128 threads per 16x16 tile; a thread owns 2 vertically adjacent pixels, a warp an 8x8
+// block (PixelMap, render_common.cuh).  The tile's slice of the sorted instance list is consumed in
+// rounds of 128 instances, one per thread: each thread loads its instance's 32-byte projected record
+// and colour into registers a round ahead and writes them to a double buffer in shared memory when
+// the round starts, so the loads of round r+1 overlap the blending of round r.  Colours are staged
+// too (the reference fetches them from global memory inside the blend loop, forward.cu:376).
 //
-// Per-warp culling: before blending a round, every lane tests 8 of the 256 staged Gaussians against the
+// Per-warp culling: before blending 32 staged Gaussians, every lane tests one of them against the
 // bounding box of the warp's sample positions using the conservative footprint extents computed in
 // preprocess_fwd.cu, then against the footprint ellipse itself (ellipse_may_touch, render_common.cuh);
-// eight ballots give the warp a 256-bit mask and only the set bits are blended.
+// a ballot gives the warp a 32-bit mask and only the set bits are blended.
 // The skipped (pixel, Gaussian) pairs are pairs the reference rejects with alpha < 1/255
 // (forward.cu:365), so the image, final_T and n_contrib are unchanged; `contributor` is derived from
 // the position in the list, not counted, so it still counts every instance like forward.cu:349.
 //
-// Blend masks: for the first MASK_K positions of a tile's list, every kernel records per 8x8 pixel
-// block whether some pixel of the block blended the position (common.cuh).  The backward walks only
-// those positions.
+// Blend masks: for the first MASK_K positions of a tile's list, the training composite records per
+// 8x8 pixel block whether some pixel of the block blended the position (common.cuh).  The backward
+// walks only those positions.
 //
-// Numerics contract (SURVEY.md 8a note N3): the expression shapes of power / alpha / test_T / the
-// colour accumulation are exactly the reference's (forward.cu:353-378,393), and expf is the accurate
-// one, so the three discontinuous tests (power > 0, alpha < 1/255, T(1-alpha) < 1e-4) take the same
-// branch and n_contrib / pixels match bit for bit.
+// Numerics contract (SURVEY.md 8a note N3): power / alpha / test_T / the colour accumulation have
+// the reference's expression shapes (forward.cu:353-378,393), fused exactly where nvcc fuses the
+// reference's scalar expressions; every other operation is rounded as its scalar instruction and never
+// contracted (add2 / mul2, render_common.cuh), and expf is the accurate one.  So the three
+// discontinuous tests (power > 0, alpha < 1/255, T(1-alpha) < 1e-4) take the reference's branch and
+// n_contrib / pixels match the reference bit for bit.
 #include "render_common.cuh"
-#include <cstdlib>
 
 namespace gsr {
 
@@ -59,189 +60,14 @@ __device__ __forceinline__ uint32_t* blend_mask_word(const RenderFwdParams& p, i
     return p.blend_mask + ((size_t)tile * MASK_BLOCKS + k) * MASK_WORDS + word;
 }
 
-template <int PPT>
-__global__ void __launch_bounds__(PixelMap<PPT>::THREADS) render_fwd_kernel(const __grid_constant__ RenderFwdParams p) {
-    using PM = PixelMap<PPT>;
-    static_assert(PPT == 1, "the blend-mask combine below assumes 8 warps of 8x4 pixels");
-    constexpr int THREADS = PM::THREADS;
-    __shared__ __align__(16) float4 s_geo[2][RT_BATCH];   // {x, y, hx, hy}
-    __shared__ __align__(16) float4 s_con[2][RT_BATCH];   // {conic.x, conic.y, conic.z, opacity}
-    __shared__ __align__(16) float4 s_col[2][RT_BATCH];   // {r, g, b, -}
-    __shared__ uint32_t s_blend[PM::WARPS][RT_BATCH / 32];   // this round's blend-mask words of each warp
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
-
-    float2 pixf[PPT];
-    unsigned pix_id[PPT];
-    bool inside[PPT];
-    unsigned live = 0;          // bit k set: pixel k still compositing
-    float bx0 = 3.0e38f, bx1 = -3.0e38f, by0 = 3.0e38f, by1 = -3.0e38f;
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        int lx, ly;
-        PM::pixel(tid, k, lx, ly);
-        const unsigned px = tile_x * TILE + lx, py = tile_y * TILE + ly;
-        pix_id[k] = p.W * py + px;
-        inside[k] = px < (unsigned)p.W && py < (unsigned)p.H;
-        pixf[k] = {(float)px, (float)py};
-        if (inside[k]) {
-            const float2 so = p.subpixel_offset[pix_id[k]];
-            pixf[k].x += so.x;
-            pixf[k].y += so.y;
-            live |= 1u << k;
-            bx0 = fminf(bx0, pixf[k].x); bx1 = fmaxf(bx1, pixf[k].x);
-            by0 = fminf(by0, pixf[k].y); by1 = fmaxf(by1, pixf[k].y);
-        }
-    }
-    const WarpBox box = warp_box_reduce(bx0, bx1, by0, by1);
-
-    const uint2 range = p.ranges[tile_y * p.grid_x + tile_x];
-    const int total = (int)(range.y - range.x);
-    const int rounds = (total + RT_BATCH - 1) / RT_BATCH;
-
-    // gather of one round into buffer `buf`; ids were loaded one iteration earlier
-    auto stage = [&](int buf, int round, const uint32_t (&ids)[PPT]) {
-#pragma unroll
-        for (int q = 0; q < PPT; ++q) {
-            const int slot = q * THREADS + tid;
-            if (round * RT_BATCH + slot < total) {
-                const float4* src = p.rec + 2 * (size_t)ids[q];
-                cp_async_16(&s_geo[buf][slot], src);
-                cp_async_16(&s_con[buf][slot], src + 1);
-                const float* c = p.colors + 3 * (size_t)ids[q];
-                float* cdst = reinterpret_cast<float*>(&s_col[buf][slot]);
-                cp_async_4(cdst, c);
-                cp_async_4(cdst + 1, c + 1);
-                cp_async_4(cdst + 2, c + 2);
-            }
-        }
-    };
-    auto load_ids = [&](int round, uint32_t (&ids)[PPT]) {
-#pragma unroll
-        for (int q = 0; q < PPT; ++q) {
-            const int i = round * RT_BATCH + q * THREADS + tid;
-            ids[q] = (round < rounds && i < total) ? p.point_list[range.x + i] : 0u;
-        }
-    };
-
-    float T[PPT], C0[PPT], C1[PPT], C2[PPT];
-    uint32_t last_contributor[PPT];
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) { T[k] = 1.0f; C0[k] = C1[k] = C2[k] = 0.f; last_contributor[k] = 0; }
-
-    if (rounds > 0) {
-        uint32_t ids[PPT];
-        load_ids(0, ids);
-        stage(0, 0, ids);
-        cp_async_commit();
-        load_ids(1, ids);
-
-        int toDo = total;
-        for (int r = 0; r < rounds; ++r, toDo -= RT_BATCH) {
-            const int buf = r & 1;
-            // this round's data has landed (for this thread) ...
-            cp_async_wait<0>();
-            // ... and for everyone; also the block-wide early-out vote (forward.cu:330-332)
-            const int num_done = __syncthreads_count(live == 0);
-            if (num_done == THREADS) break;
-            // next round's gather overlaps this round's blending
-            if (r + 1 < rounds) {
-                stage(buf ^ 1, r + 1, ids);
-                cp_async_commit();
-                load_ids(r + 2, ids);
-            }
-
-            const int n = min(RT_BATCH, toDo);
-            const uint32_t round_base = (uint32_t)(r * RT_BATCH);
-            uint32_t my_word = 0;   // lane w holds the blend-mask word of the round's batch w
-            if (__any_sync(0xFFFFFFFFu, live != 0)) {
-                // which of the staged Gaussians can touch this warp's pixels?  32 at a time: one ballot, then only
-                // the set bits are blended
-#pragma unroll 1
-                for (int w = 0; w < RT_BATCH / 32; ++w) {
-                    const int jl = w * 32 + lane;
-                    bool rel = false;
-                    if (jl < n) {
-                        const float4 g = s_geo[buf][jl], c = s_con[buf][jl];
-                        rel = box_may_touch(g, box) && ellipse_may_touch(g.x, g.y, c.x, c.y, c.z, c.w, box);
-                    }
-                    unsigned mm = __ballot_sync(0xFFFFFFFFu, rel);
-                    uint32_t blended = 0;
-                    while (mm) {
-                        const int j = w * 32 + __ffs(mm) - 1;
-                        mm &= mm - 1;
-                        const float4 geo = s_geo[buf][j];
-                        const float4 con_o = s_con[buf][j];
-                        bool upd = false;
-#pragma unroll
-                        for (int k = 0; k < PPT; ++k) {
-                            if (!(live & (1u << k))) continue;
-                            const float2 xy = {geo.x, geo.y};
-                            const float2 d = {xy.x - pixf[k].x, xy.y - pixf[k].y};
-                            const float power = -0.5f * (con_o.x * d.x * d.x + con_o.z * d.y * d.y) - con_o.y * d.x * d.y;
-                            if (power > 0.0f) continue;
-
-                            const float alpha = min(0.99f, con_o.w * expf(power));
-                            if (alpha < 1.0f / 255.0f) continue;
-                            const float test_T = T[k] * (1 - alpha);
-                            if (test_T < 0.0001f) {
-                                live &= ~(1u << k);
-                                continue;
-                            }
-                            const float4 col = s_col[buf][j];
-                            C0[k] += col.x * alpha * T[k];
-                            C1[k] += col.y * alpha * T[k];
-                            C2[k] += col.z * alpha * T[k];
-                            T[k] = test_T;
-                            // 1-based position of this instance in the tile's list (forward.cu:349,382)
-                            last_contributor[k] = round_base + (uint32_t)j + 1u;
-                            upd = true;
-                        }
-                        if (__any_sync(0xFFFFFFFFu, upd)) blended |= 1u << (j - w * 32);
-                    }
-                    if (lane == w) my_word = blended;
-                    if (!__any_sync(0xFFFFFFFFu, live != 0)) break;
-                }
-            }
-            if (lane < RT_BATCH / 32) s_blend[warp][lane] = my_word;
-            // everyone is finished with `buf` before round r+2 is staged into it
-            __syncthreads();
-            // an 8x8 block is two 8x4 warp blocks (warps wa and wa + 2): its words are the OR of theirs.  s_blend is
-            // rewritten only after the next round's barrier.
-            if (tid < MASK_BLOCKS * (RT_BATCH / 32)) {
-                const int k = tid / (RT_BATCH / 32), i = tid % (RT_BATCH / 32);
-                const int wa = (k & 1) + 4 * (k >> 1);
-                const int word = r * (RT_BATCH / 32) + i;
-                if (word < MASK_WORDS) *blend_mask_word(p, k, word) = s_blend[wa][i] | s_blend[wa + 2][i];
-            }
-        }
-        cp_async_wait<0>();
-    }
-
-    const size_t plane = (size_t)p.H * p.W;
-    const float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        if (inside[k]) {
-            p.final_T[pix_id[k]] = T[k];
-            p.n_contrib[pix_id[k]] = last_contributor[k];
-            p.out_color[0 * plane + pix_id[k]] = C0[k] + T[k] * bg0;
-            p.out_color[1 * plane + pix_id[k]] = C1[k] + T[k] * bg1;
-            p.out_color[2 * plane + pix_id[k]] = C2[k] + T[k] * bg2;
-        }
-    }
-}
-
-// ---- packed variant: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2) ----------------
-// (see render_bwd.cu: both pixels of a lane share every per-Gaussian operand load and the loop control.)  Every element of a pair goes through the same
-// IEEE operations, in the same order, as the scalar kernel above -- power = fma(fma(dx, A dx, (C dy) dy), -0.5,
-// -((B dx) dy)), alpha = min(0.99, o expf(power)), test_T = T (1 - alpha), C = fma(T, alpha c, C) -- so pixels,
-// final_T and n_contrib are bit-identical.  A pair that does not blend is carried as alpha = 0, which leaves C and T
-// unchanged exactly.
-// Staging: one instance per thread and round; the raw records travel through registers (loads of round r+1 are
-// issued before round r is blended) and are written to shared memory already duplicated ({x, x, y, y}, ...), so one
-// LDS.128 yields two ready-made broadcast pairs.
+// ---- packed composite: 2 pixels per lane, their arithmetic written as pairs (add2 / mul2 / fma2) ----------------
+// Both pixels of a lane share every per-Gaussian operand load and the loop control.  Each element of a pair goes through
+// the reference's operations in the reference's order (forward.cu:353-378) -- power = fma(fma(dx, A dx, (C dy) dy),
+// -0.5, -((B dx) dy)), alpha = min(0.99, o expf(power)), test_T = T (1 - alpha), C = fma(T, alpha c, C) -- so pixels,
+// final_T and n_contrib are the reference's bits.  A pair that does not blend is carried as alpha = 0, which leaves C
+// and T unchanged exactly.
+// Staging: the raw records travel through registers and are written to shared memory already duplicated
+// ({x, x, y, y}, ...), so one LDS.128 yields two ready-made broadcast pairs.
 struct __align__(16) FwdPairRec {     // 80 bytes
     float4 xy;     // {x, x, y, y}
     float4 ac;     // {conic.x, conic.x, conic.z, conic.z}
@@ -263,12 +89,12 @@ __device__ __forceinline__ float display_value(float x) { return isnan(x) ? 0.f 
 template <bool DISPLAY, bool DEPTH>
 __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_constant__ RenderFwdParams p) {
     static_assert(DISPLAY || !DEPTH, "the depth channel is a display output");
-    using PM = PixelMap<2>;
+    using PM = PixelMap;
     constexpr int THREADS = 128;
     constexpr int PB = 128;               // instances per round
     __shared__ FwdPairRec s_rec[2][PB];
-    __shared__ uint32_t s_blend[PixelMap<2>::WARPS][MASK_WORDS];   // blend-mask words, written out at the end
-    __shared__ float2 s_dep[2][DEPTH ? PB : 1];                    // {d, d} of the depth channel
+    __shared__ uint32_t s_blend[PixelMap::WARPS][MASK_WORDS];   // blend-mask words, written out at the end
+    __shared__ float2 s_dep[2][DEPTH ? PB : 1];                 // {d, d} of the depth channel
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int tile_x = blockIdx.x, tile_y = blockIdx.y + p.ty0;
@@ -410,7 +236,7 @@ __global__ void __launch_bounds__(128, 9) render_fwd_packed_kernel(const __grid_
         }
     }
 
-    // PixelMap<2>: warp k is 8x8 block k.  Words of batches no warp entered are copied too; they are never read.
+    // PixelMap: warp k is 8x8 block k.  Words of batches no warp entered are copied too; they are never read.
     if constexpr (!DISPLAY) {
         __syncthreads();
         for (int i = tid; i < MASK_BLOCKS * MASK_WORDS; i += THREADS)
@@ -490,7 +316,7 @@ __device__ __forceinline__ float butterfly3(float v0, float v1, float v2, int la
 }
 
 __global__ void __launch_bounds__(128) render_color_grad_kernel(const __grid_constant__ ColorGradParams p) {
-    using PM = PixelMap<2>;
+    using PM = PixelMap;
     constexpr int WARPS = PM::WARPS;
     constexpr int PB = 128;               // instances per round (one per thread)
     constexpr int NW = PB / 32;           // blend-mask words per round (rounds start at multiples of 32 positions)
@@ -637,17 +463,7 @@ int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinStat
     p.peer_out = (float* const*)(a.peer_images); p.n_peers = a.n_peer_images;
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);
-    static int packed = -1;
-    if (packed < 0) {
-        const char* e = getenv("GSR_FWD_PACKED");     // tuning aid: 1 = 2 pixels/lane in paired fp32 instructions
-        packed = e ? atoi(e) : 1;
-    }
-    if (packed || p.n_peers > 0) {      // the fused all-gather epilogue exists in the packed kernel only
-        render_fwd_packed_kernel<false, false><<<grid, 128, 0, s>>>(p);
-        count_launches(1);
-        return 0;
-    }
-    render_fwd_kernel<1><<<grid, PixelMap<1>::THREADS, 0, s>>>(p);
+    render_fwd_packed_kernel<false, false><<<grid, 128, 0, s>>>(p);
     count_launches(1);
     return 0;
 }
