@@ -358,8 +358,8 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
 
                 const float4 rg = R.rg, bk = R.bk;
                 const float2 oma = add2(one, make_float2(-alpha.x, -alpha.y));
-                // T before this splat; 1 - alpha is in [0.01, 1], the approximate reciprocal is good to 1 ulp and gradients
-                // are compared at 1e-3 (backward.cu:548,579 divide twice)
+                // T before this splat; 1 - alpha is in [0.01, 1], the approximate reciprocal is good to 1 ulp, an error
+                // the per-entry bound of oracle/bwd_bound.c carries (backward.cu:548,579 divide twice)
                 const float2 inv = make_float2(rcp_approx(oma.x), rcp_approx(oma.y));
                 T = mul2(T, inv);
                 const float2 aT = mul2(alpha, T);
