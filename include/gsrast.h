@@ -170,19 +170,6 @@ int gsr_forward_render(const GsrForwardArgs* args, void* geom_buffer, void* img_
                        void* stream);
 int gsr_forward(const GsrForwardArgs* args, gsr_alloc_fn alloc, void* alloc_ctx,
                 void* stream, int* num_rendered);
-/* The whole forward WITHOUT the host synchronisation in its middle (the reference blocks on the instance count at
- * rasterizer_impl.cu:283-284, gsr_forward_geometry does the same): the caller supplies the binning buffer and the
- * scratch sized for `rendered_capacity` instances / `coarse_capacity` coarse items (gsr_binning_sizes; typically the
- * previous frame's counts plus a margin), every launch configuration is derived from the capacities and the actual
- * counts stay on the device.  If the scene does not fit, the binning / composite stages turn into no-ops (empty tile
- * lists, no out-of-bounds access) and an overflow flag is raised.  gsr_forward_status() -- one stream synchronisation,
- * whenever the caller needs the counts -- returns the exact num_rendered / num_coarse (valid even after an overflow, so
- * one retry with exactly sized buffers, e.g. through gsr_forward_geometry + gsr_forward_render, always succeeds) and
- * overflow != 0 if the forward must be repeated.  CUDA-graph capturable (no synchronisation, fixed launch shapes).    */
-int gsr_forward_async(const GsrForwardArgs* args, void* geom_buffer, void* img_buffer, void* binning_buffer,
-                      int rendered_capacity, void* scratch, int coarse_capacity, void* stream);
-int gsr_forward_status(const void* geom_buffer, int P, int M, void* stream, int* num_rendered, int* num_coarse,
-                       int* overflow);
 
 /* Re-composite with different per-Gaussian colours on the SAME geometry/binning state
  * (wild-gaussians renders raw + appearance-toned colours per step, method.py:1573-1611).

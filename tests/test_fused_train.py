@@ -534,7 +534,7 @@ class _CountingLib:
 
     def __getattr__(self, name):
         fn = getattr(self.lib, name)
-        if name in ("gsr_forward_geometry", "gsr_forward_status"):
+        if name == "gsr_forward_geometry":
             def counted(*a, **k):
                 self.readbacks += 1
                 return fn(*a, **k)

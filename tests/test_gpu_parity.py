@@ -513,32 +513,44 @@ def test_geometry_cache_hits_with_a_non_contiguous_view_matrix(C, dev):
     assert C.geometry_cache_hits() == h0 + 2                    # (run_ours' forward hit too) the entry was released when its backward started
 
 
-def test_async_forward_capacity_overflow_is_retried(C, dev):
-    """The sync-free forward runs on buffers sized from the previous call's counts.  When the scene outgrows them the
-    device raises an overflow flag (no out-of-bounds access: binning and composite become no-ops) and the host repeats
-    binning + composite with exactly sized buffers: results are identical to a first (two-phase) call."""
-    scene = synthetic.make_scene(P=60_000, W=480, H=320, sh_degree=None, seed=52)
+def test_render_counts_too_small_for_the_scene_render_nothing(C, dev):
+    """gsr_forward_render takes the instance and coarse-item counts from its caller.  Counts smaller than the scene's
+    bin nothing (empty tile ranges, no write beyond the buffers sized for them) and leave the background; a following
+    call with the right counts on the same geometry is bit-identical to the ordinary forward."""
+    from ctypes import byref, c_size_t
+    scene = synthetic.make_scene(P=60_000, W=480, H=320, sh_degree=None, seed=52, bg=(0.2, 0.1, 0.3))
     d = synthetic.to_device(scene, dev)
     C.set_geometry_cache(False)
-    C.set_async_forward(True)
-    C._size_hint.clear()
-    first = run_ours(C, d)                                   # no hint: gsr_forward_geometry + gsr_forward_render
-    key = next(iter(C._size_hint))
-    assert C._size_hint[key][0] >= first["R"]
-    second = run_ours(C, d)                                  # hint: gsr_forward_async
-    for k in ("point_list", "ranges", "n_contrib"):
-        assert torch.equal(first["views"][k], second["views"][k]), k
-    assert torch.equal(first["color"], second["color"]) and first["R"] == second["R"]
-    n0 = C._counters.get("overflow_retries", 0)
-    for caps in ((first["R"] // 2, 10**8), (10**8, 100), (0, 0), (1, 1)):
-        C._size_hint[key] = caps                             # instance capacity / coarse capacity too small
-        o = run_ours(C, d)
-        assert torch.equal(o["color"], first["color"]) and o["R"] == first["R"]
-        assert torch.equal(o["views"]["point_list"], first["views"]["point_list"])
-        for n in ("dL_dmeans3D", "dL_dcolors"):
-            assert rel_err(o["grads"][n].cpu().numpy(), first["grads"][n].cpu().numpy()) < 1e-5
-    assert C._counters.get("overflow_retries", 0) == n0 + 4
-    C.set_async_forward(False)
+    want = run_ours(C, d)
+    P, W, H = d["means3D"].shape[0], d["image_width"], d["image_height"]
+    out_color, radii = torch.empty((3, H, W), device=dev), torch.empty((P,), dtype=torch.int32, device=dev)
+    a = C.forward_args(background=d["bg"], means3D=d["means3D"], colors=d["colors_precomp"], opacities=d["opacities"],
+                       scales=d["scales"], rotations=d["rotations"], viewmatrix=d["viewmatrix"],
+                       projmatrix=d["projmatrix"], campos=d["campos"], tan_fovx=d["tanfovx"], tan_fovy=d["tanfovy"],
+                       kernel_size=d["kernel_size"], subpixel_offset=d["subpixel_offset"], H=H, W=W, radii=radii,
+                       out_color=out_color)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    geom, img, binning, scratch, R, N1 = C._forward_geometry(a, dev, stream)
+    assert R == want["R"] and R > 1 and N1 > 1
+    for r, n1 in ((1, 1), (0, 0)):
+        bb, sb = c_size_t(0), c_size_t(0)
+        C._check(C._lib.gsr_binning_sizes(P, W, H, r, n1, byref(bb), byref(sb)), "gsr_binning_sizes")
+        small_bin = torch.empty((bb.value,), dtype=torch.uint8, device=dev)
+        small_scratch = torch.empty((sb.value,), dtype=torch.uint8, device=dev)
+        out_color.fill_(float("nan"))
+        C._check(C._lib.gsr_forward_render(byref(a), geom.data_ptr(), img.data_ptr(), small_bin.data_ptr(),
+                                           small_scratch.data_ptr(), r, n1, stream), "gsr_forward_render")
+        ranges = C.debug_views(geom, small_bin, img, P, 0, W, H, 0)["ranges"]
+        torch.cuda.synchronize()
+        assert torch.equal(ranges[:, 0], ranges[:, 1]), (r, n1)
+        assert torch.equal(out_color, d["bg"].view(3, 1, 1).expand(3, H, W)), (r, n1)
+    C._check(C._lib.gsr_forward_render(byref(a), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), scratch.data_ptr(),
+                                       R, N1, stream), "gsr_forward_render")
+    v = C.debug_views(geom, binning, img, P, 0, W, H, R)
+    torch.cuda.synchronize()
+    assert torch.equal(out_color, want["color"]) and torch.equal(radii, want["radii"])
+    for k in ("point_list", "ranges", "n_contrib", "final_T"):
+        assert torch.equal(v[k], want["views"][k]), k
     C.set_geometry_cache(True)
 
 

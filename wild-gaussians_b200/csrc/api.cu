@@ -345,45 +345,6 @@ int gsr_forward_render(const GsrForwardArgs* a, void* geom_buffer, void* img_buf
     return binning_and_render(a, g, im, b, bs, (size_t)num_rendered, (size_t)num_coarse, ty0, ty1, (cudaStream_t)stream);
 }
 
-int gsr_forward_async(const GsrForwardArgs* a, void* geom_buffer, void* img_buffer, void* binning_buffer,
-                      int rendered_capacity, void* scratch, int coarse_capacity, void* stream) {
-    int rc = check_fwd_args(a);
-    if (rc) return rc;
-    if (a->P == 0) return 0;
-    if (!geom_buffer || !img_buffer || rendered_capacity < 0 || coarse_capacity < 0 ||
-        ((rendered_capacity > 0 && coarse_capacity > 0) && (!binning_buffer || !scratch))) {
-        set_error("a buffer is NULL or a capacity is negative");
-        return GSR_E_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    GeomState g;
-    ImgState im;
-    BinState b;
-    BinScratch bs;
-    carve_geom((char*)geom_buffer, a->P, a->M, &g);
-    carve_img((char*)img_buffer, a->W, a->H, &im);
-    carve_bin((char*)binning_buffer, (size_t)rendered_capacity, &b);
-    carve_bin_scratch((char*)scratch, (size_t)coarse_capacity, a->W, a->H, &bs);
-    int ty0, ty1;
-    shard_rows(a->H, a->tile_y0, a->tile_y1, &ty0, &ty1);
-    rc = geometry_stage(a, g, ty0, ty1, s);
-    if (rc) return rc;
-    return binning_and_render(a, g, im, b, bs, (size_t)rendered_capacity, (size_t)coarse_capacity, ty0, ty1, s);
-}
-
-int gsr_forward_status(const void* geom_buffer, int P, int M, void* stream, int* num_rendered, int* num_coarse, int* overflow) {
-    if (!geom_buffer || !num_rendered || !num_coarse || !overflow) { set_error("NULL argument"); return GSR_E_INVALID; }
-    *num_rendered = *num_coarse = *overflow = 0;
-    if (P == 0) return 0;
-    GeomState g;
-    carve_geom((char*)geom_buffer, P, M, &g);
-    int32_t c[8];
-    int rc = read_counters(g, (cudaStream_t)stream, c);
-    if (rc) return rc;
-    *overflow = c[6];
-    return counts_of(c, num_rendered, num_coarse);
-}
-
 int gsr_forward(const GsrForwardArgs* a, gsr_alloc_fn alloc, void* ctx, void* stream, int* num_rendered) {
     int rc = check_fwd_args(a);
     if (rc) return rc;

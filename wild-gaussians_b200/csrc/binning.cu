@@ -30,10 +30,10 @@ namespace gsr {
 // ---- level 1: coarse items ------------------------------------------------------------------------
 // key = cell id (low 16 bits) | x0 << 16 | y0 << 20 | x1 << 24 | y1 << 28, rectangle local to the cell
 // counters (GeomState::counters): [2..3] R = exact instance count of the band (u64, preprocess), [4] N1 = coarse
-// items (scan total), [5] number of depth-sorted Gaussians, [6] overflow flags, [7] N1 if everything fits the supplied
-// buffers, else 0 -- the item count every later binning kernel works with, so that an overflow turns the rest of
-// the forward into a harmless no-op (empty tile ranges) instead of writing out of bounds; the host re-runs with
-// exact sizes when it sees the flag.
+// items (scan total), [5] number of depth-sorted Gaussians, [7] N1 if the scene fits the counts the binning buffers
+// were sized for, else 0 -- the item count every later binning kernel works with.  gsr_forward_render and
+// gsr_forward_display take those counts from the caller: counts smaller than the scene's turn the rest of the forward
+// into a harmless no-op (empty tile ranges) instead of writing out of bounds.
 __global__ void __launch_bounds__(256) emit_cells_kernel(int cells_x, const uint32_t* __restrict__ order,
                                                          const uint32_t* __restrict__ offsets,
                                                          const TileRect* __restrict__ rect,
@@ -43,10 +43,7 @@ __global__ void __launch_bounds__(256) emit_cells_kernel(int cells_x, const uint
     const uint32_t n1 = (uint32_t)counters[4];
     const unsigned long long R = *reinterpret_cast<const unsigned long long*>(counters + 2);
     const bool fits = n1 <= n1_cap && R <= r_cap;
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        counters[7] = fits ? (int32_t)n1 : 0;
-        if (!fits) counters[6] = (n1 > n1_cap ? 1 : 0) | (R > r_cap ? 2 : 0);
-    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) counters[7] = fits ? (int32_t)n1 : 0;
     if (!fits) return;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;   // position in depth order
     if (i >= (uint32_t)counters[5]) return;
@@ -427,10 +424,8 @@ int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R_cap, size
     const uint32_t num_cells = (uint32_t)(cells_x * cells_y);
     const int num_tiles = gx * gy;
     if (N1_cap == 0 || R_cap == 0) {
-        // nothing can be binned: empty ranges; a non-empty scene then shows up as an overflow (flags set by this kernel)
+        // nothing can be binned: empty ranges
         GSR_CUDA(cudaMemsetAsync(ranges, 0, (size_t)num_tiles * sizeof(uint2), s));
-        emit_cells_kernel<<<1, 32, 0, s>>>(cells_x, g.order, g.offsets, g.rect_sorted, nullptr, nullptr, g.counters, 0u, 0ull);
-        count_launches(1);
         return 0;
     }
     // level 1: emit + stable sort by cell id; the sorted result must land in (key_b, val_b)

@@ -130,8 +130,6 @@ def _load():
     lib.gsr_forward_geometry.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, POINTER(c_int), POINTER(c_int)]
     lib.gsr_binning_sizes.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t)]
     lib.gsr_forward_render.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]
-    lib.gsr_forward_async.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
-    lib.gsr_forward_status.argtypes = [c_void_p, c_int, c_int, c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int)]
     lib.gsr_forward_recolor.argtypes = [POINTER(GsrForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.gsr_forward_display.argtypes = [POINTER(GsrForwardArgs), POINTER(GsrDisplayArgs), c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_int, c_int, c_void_p]
@@ -233,7 +231,7 @@ def _load():
     lib.gsr_profile_read.argtypes = [POINTER(c_float), c_int]
     lib.gsr_launch_count.restype = ctypes.c_ulonglong
     for name in ("gsr_forward_sizes", "gsr_forward_geometry", "gsr_binning_sizes", "gsr_forward_render",
-                 "gsr_forward_recolor", "gsr_forward_async", "gsr_forward_status", "gsr_backward", "gsr_backward_partials", "gsr_backward_finalize",
+                 "gsr_forward_recolor", "gsr_backward", "gsr_backward_partials", "gsr_backward_finalize",
                  "gsr_backward_partials_peers",
                  "gsr_mark_visible", "gsr_img_views", "gsr_binning_views",
                  "gsr_geom_views", "gsr_get_stats"):
@@ -265,23 +263,9 @@ def get_tile_row_shard():
 # version counter (no in-place modification since), on the same stream, with the same scalar settings.  The entry
 # keeps those tensors and their converted copies alive, so their addresses cannot be recycled for other data.
 # Modifying a tensor behind autograd's back (``x.data.add_(...)``, a raw kernel writing through data_ptr) does not
-# bump the version: call clear_geometry_cache() after such writes or set GSR_GEOM_CACHE=0.  The entry is dropped when
-# a backward pass starts (no further forward on this geometry can follow before the parameters change).
-_size_hint: dict = {}      # (P, W, H, shard) -> (instance capacity, coarse-item capacity) for the next call
-_counters: dict = {}       # bookkeeping: "overflow_retries"
-# GSR_ASYNC_FORWARD=1: enqueue the whole forward on capacity-sized buffers and read the counts back at its END
-# (gsr_forward_async + gsr_forward_status) instead of the two-phase protocol with the read-back in the middle.  Off by
-# default: in a training loop the two-phase read-back costs one ~10 us bubble per step (everything after it is already
-# queued behind the GPU), whereas a synchronisation at the end of the forward exposes the host-side work between the
-# forward and the backward (measured at C3: 1.75 ms/step two-phase, 1.79 ms/step with the end-of-forward read-back).
-# The asynchronous entry point is what a CUDA-graph capture of the forward needs.
-_ASYNC_FORWARD = os.environ.get("GSR_ASYNC_FORWARD", "0") != "0"
-
-
-def set_async_forward(on: bool) -> None:
-    global _ASYNC_FORWARD
-    _ASYNC_FORWARD = bool(on)
-_GEOM_CACHE_ON = os.environ.get("GSR_GEOM_CACHE", "1") != "0"
+# bump the version: call clear_geometry_cache() after such writes or set_geometry_cache(False).  The entry is dropped
+# when a backward pass starts (no further forward on this geometry can follow before the parameters change).
+_GEOM_CACHE_ON = True
 _geom_cache: dict = {}
 
 
@@ -332,6 +316,48 @@ def _f32c(t: torch.Tensor, device) -> torch.Tensor:
 
 def _stream(device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
+
+
+def forward_args(*, background, means3D, colors, opacities, scales, rotations, viewmatrix, projmatrix, campos, tan_fovx,
+                 tan_fovy, kernel_size, subpixel_offset, H, W, radii, out_color=None, scale_modifier=1.0,
+                 cov3D_precomp=None, sh=None, degree=0, prefiltered=False, debug=False, shard=(0, 0), peer_images=None):
+    """``GsrForwardArgs`` of contiguous fp32 tensors on one device.  None or a zero-element tensor (the reference's
+    "absent" input) becomes NULL; P is the number of rows of ``means3D``, M the number of SH coefficients of ``sh``.
+    ``shard`` is in the ABI's form (``_abi_shard``), ``peer_images = (device address of the array of per-rank image
+    pointers, number of ranks)``."""
+    a = GsrForwardArgs()
+    a.P, a.D, a.W, a.H = int(means3D.size(0)), int(degree), int(W), int(H)
+    a.M = int(sh.size(1)) if sh is not None and sh.numel() != 0 else 0
+    a.background, a.means3D, a.shs, a.colors_precomp = _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors)
+    a.opacities, a.scales, a.rotations = _ptr(opacities), _ptr(scales), _ptr(rotations)
+    a.scale_modifier, a.cov3D_precomp = float(scale_modifier), _ptr(cov3D_precomp)
+    a.viewmatrix, a.projmatrix, a.campos = _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos)
+    a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
+    a.subpixel_offset = _ptr(subpixel_offset)
+    a.prefiltered, a.debug = int(bool(prefiltered)), int(bool(debug))
+    a.tile_y0, a.tile_y1 = shard
+    a.out_color, a.radii = _ptr(out_color), _ptr(radii)
+    if peer_images is not None:
+        a.peer_images, a.n_peer_images = int(peer_images[0]), int(peer_images[1])
+    return a
+
+
+def _forward_geometry(a, dev, stream):
+    """First phase of the forward, shared by the training composite (``gsr_forward_render``) and the display composite
+    (``gsr_forward_display``): allocates the geometry and image buffers, runs projection, depth ordering and the
+    coarse-item offsets (``gsr_forward_geometry``, whose instance-count read-back is the forward's host
+    synchronisation) and allocates the binning buffers for those counts.  Returns ``(geom, img, binning, scratch, R,
+    N1)``."""
+    byte = dict(dtype=torch.uint8, device=dev)
+    gb, ib = c_size_t(0), c_size_t(0)
+    _check(_lib.gsr_forward_sizes(a.P, a.M, a.W, a.H, byref(gb), byref(ib)), "gsr_forward_sizes")
+    geom, img = torch.empty((gb.value,), **byte), torch.empty((ib.value,), **byte)
+    R, N1 = c_int(0), c_int(0)
+    _check(_lib.gsr_forward_geometry(byref(a), geom.data_ptr(), img.data_ptr(), stream, byref(R), byref(N1)),
+           "gsr_forward_geometry")
+    bb, sb = c_size_t(0), c_size_t(0)
+    _check(_lib.gsr_binning_sizes(a.P, a.W, a.H, R.value, N1.value, byref(bb), byref(sb)), "gsr_binning_sizes")
+    return geom, img, torch.empty((bb.value,), **byte), torch.empty((sb.value,), **byte), R.value, N1.value
 
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
@@ -404,8 +430,6 @@ def rasterize_gaussians_shard(shard, background, means3D, colors, opacity, scale
         out_color = None if peer_images is not None else alloc_img((NUM_CHANNELS, H, W), dtype=torch.float32, device=dev)
         M = int(sh.size(1)) if sh.numel() != 0 else 0
         stream = _stream(dev)
-        gb, ib = c_size_t(0), c_size_t(0)
-        _check(_lib.gsr_forward_sizes(P, M, W, H, byref(gb), byref(ib)), "gsr_forward_sizes")
 
         # Geometry reuse (SURVEY.md 8f-1): wild-gaussians composites the SAME Gaussians two or three times per step
         # with different colours (raw / appearance-toned / depth; method.py:1573-1631).  When every geometry input is
@@ -430,72 +454,29 @@ def rasterize_gaussians_shard(shard, background, means3D, colors, opacity, scale
                  background, means3D, colors, opacity, scales, rotations, cov3D_precomp, viewmatrix, projmatrix,
                  subpixel_offset, sh, campos))
 
-        a = GsrForwardArgs()
-        a.P, a.D, a.M, a.W, a.H = P, int(degree), M, W, H
-        a.background = _ptr(background); a.means3D = _ptr(means3D); a.shs = _ptr(sh)
-        a.colors_precomp = _ptr(colors); a.opacities = _ptr(opacity); a.scales = _ptr(scales)
-        a.scale_modifier = float(scale_modifier); a.rotations = _ptr(rotations)
-        a.cov3D_precomp = _ptr(cov3D_precomp); a.viewmatrix = _ptr(viewmatrix); a.projmatrix = _ptr(projmatrix)
-        a.campos = _ptr(campos); a.tan_fovx = float(tan_fovx); a.tan_fovy = float(tan_fovy)
-        a.kernel_size = float(kernel_size); a.subpixel_offset = _ptr(subpixel_offset)
-        a.prefiltered = int(bool(prefiltered)); a.debug = int(bool(debug))
-        a.tile_y0, a.tile_y1 = shard
-        a.out_color = None if out_color is None else out_color.data_ptr()
-        if peer_images is not None:
-            a.peer_images, a.n_peer_images = int(peer_images[0]), int(peer_images[1])
+        radii = hit["radii"] if hit is not None else torch.empty((P,), dtype=torch.int32, device=dev)
+        a = forward_args(background=background, means3D=means3D, colors=colors, opacities=opacity, scales=scales,
+                         rotations=rotations, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
+                         tan_fovx=tan_fovx, tan_fovy=tan_fovy, kernel_size=kernel_size, subpixel_offset=subpixel_offset,
+                         H=H, W=W, radii=radii, out_color=out_color, scale_modifier=scale_modifier,
+                         cov3D_precomp=cov3D_precomp, sh=sh, degree=degree, prefiltered=prefiltered, debug=debug,
+                         shard=shard, peer_images=peer_images)
 
         if hit is not None:
             _wait_for_composite_inputs(dev)
-            img2 = torch.empty((ib.value,), **byte)
-            a.radii = hit["radii"].data_ptr()
+            img2 = torch.empty_like(hit["img"])
             _check(_lib.gsr_forward_recolor(byref(a), hit["geom"].data_ptr(), hit["binning"].data_ptr(),
                                             hit["img"].data_ptr(), img2.data_ptr(), stream), "gsr_forward_recolor")
             _geom_cache["hits"] = _geom_cache.get("hits", 0) + 1
             # the caller gets its own radii tensor: the cached one must survive in-place edits by the caller
             return hit["R"], out_color, hit["radii"].clone(), hit["geom"], hit["binning"], img2
 
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        a.radii = radii.data_ptr()
-        geom = torch.empty((gb.value,), **byte)
-        img = torch.empty((ib.value,), **byte)
-        # Instance counts.  The reference blocks on them in the middle of its forward (rasterizer_impl.cu:283-284) and
-        # so does the two-phase protocol gsr_forward_geometry / gsr_forward_render.  When a previous call with the same
-        # shape left a capacity hint (training re-renders nearly the same scene), the whole forward is enqueued at once
-        # on buffers sized for that capacity (gsr_forward_async: no synchronisation, actual counts stay on the device)
-        # and the counts are read back once, at the END, where the caller waits for the result anyway; the GPU never
-        # idles in the middle of the forward.  If the scene outgrew the capacity the composite ran on empty tile lists:
-        # binning + composite are repeated with exactly sized buffers (the geometry stage is still valid).
-        hint_key = (P, W, H, shard)
-        hint = _size_hint.get(hint_key)
-        R, N1 = c_int(0), c_int(0)
-        bb, sb = c_size_t(0), c_size_t(0)
-        done = False
-        if hint is not None and _ASYNC_FORWARD:
-            _wait_for_composite_inputs(dev)
-            _check(_lib.gsr_binning_sizes(P, W, H, hint[0], hint[1], byref(bb), byref(sb)), "gsr_binning_sizes")
-            binning = torch.empty((bb.value,), **byte)
-            scratch = torch.empty((sb.value,), **byte)
-            _check(_lib.gsr_forward_async(byref(a), geom.data_ptr(), img.data_ptr(), binning.data_ptr(), hint[0],
-                                          scratch.data_ptr(), hint[1], stream), "gsr_forward_async")
-            ovf = c_int(0)
-            _check(_lib.gsr_forward_status(geom.data_ptr(), P, M, stream, byref(R), byref(N1), byref(ovf)),
-                   "gsr_forward_status")
-            done = ovf.value == 0
-            if not done:
-                _counters["overflow_retries"] = _counters.get("overflow_retries", 0) + 1
-        else:
-            _check(_lib.gsr_forward_geometry(byref(a), geom.data_ptr(), img.data_ptr(), stream, byref(R), byref(N1)),
-                   "gsr_forward_geometry")
-        if not done:
-            _wait_for_composite_inputs(dev)
-            _check(_lib.gsr_binning_sizes(P, W, H, R.value, N1.value, byref(bb), byref(sb)), "gsr_binning_sizes")
-            binning = torch.empty((bb.value,), **byte)
-            scratch = torch.empty((sb.value,), **byte)
-            _check(_lib.gsr_forward_render(byref(a), geom.data_ptr(), img.data_ptr(), binning.data_ptr(),
-                                           scratch.data_ptr(), R.value, N1.value, stream), "gsr_forward_render")
-        # capacity for the next call of this shape: the counts plus 1/8 (kept while the counts stay within it and above half)
-        if hint is None or R.value > hint[0] or N1.value > hint[1] or 2 * R.value < hint[0]:
-            _size_hint[hint_key] = (R.value + R.value // 8 + 4096, N1.value + N1.value // 8 + 4096)
+        # the instance counts: the reference blocks on them in the middle of its forward (rasterizer_impl.cu:283-284),
+        # and so does _forward_geometry; binning and composite follow on buffers sized for them
+        geom, img, binning, scratch, R, N1 = _forward_geometry(a, dev, stream)
+        _wait_for_composite_inputs(dev)
+        _check(_lib.gsr_forward_render(byref(a), geom.data_ptr(), img.data_ptr(), binning.data_ptr(),
+                                       scratch.data_ptr(), R, N1, stream), "gsr_forward_render")
         # `scratch` goes back to torch's stream-ordered caching allocator here: any later
         # allocation on this stream is ordered after the kernels that use it.
         del scratch
@@ -503,8 +484,8 @@ def rasterize_gaussians_shard(shard, background, means3D, colors, opacity, scale
             _geom_cache["entry"] = dict(
                 key=geo_key, orig=geo_orig,
                 conv=(means3D, opacity, scales, rotations, cov3D_precomp, viewmatrix, projmatrix, subpixel_offset),
-                R=R.value, radii=radii.clone(), geom=geom, binning=binning, img=img)
-    return R.value, out_color, radii, geom, binning, img
+                R=R, radii=radii.clone(), geom=geom, binning=binning, img=img)
+    return R, out_color, radii, geom, binning, img
 
 
 def _backward_impl(mode, accum, background, means3D, radii, colors, scales, rotations, scale_modifier,

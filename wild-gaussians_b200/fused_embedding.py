@@ -144,17 +144,11 @@ class EmbeddingLoop:
         stream = torch.cuda.current_stream(dev).cuda_stream
         self.stream = stream
 
-        fa = _C.GsrForwardArgs()
-        fa.P, fa.D, fa.M, fa.W, fa.H = P, self.deg, 0, W, H
-        fa.background, fa.means3D, fa.colors_precomp = bg.data_ptr(), model.xyz.data_ptr(), self.colors.data_ptr()
-        fa.opacities, fa.scales, fa.rotations = opacity.data_ptr(), scales.data_ptr(), rotations.data_ptr()
-        fa.scale_modifier = 1.0
-        fa.viewmatrix, fa.projmatrix = cc["world_view"].data_ptr(), cc["full_proj"].data_ptr()
-        fa.campos = cc["cam_center"].data_ptr()
-        fa.tan_fovx, fa.tan_fovy, fa.kernel_size = cc["tanfovx"], cc["tanfovy"], float(config.kernel_size)
-        fa.subpixel_offset = sub.data_ptr()
-        fa.out_color, fa.radii = self.image.data_ptr(), radii.data_ptr()
-        self.fwd_args = fa
+        self.fwd_args = _C.forward_args(
+            background=bg, means3D=model.xyz, colors=self.colors, opacities=opacity, scales=scales, rotations=rotations,
+            viewmatrix=cc["world_view"], projmatrix=cc["full_proj"], campos=cc["cam_center"], tan_fovx=cc["tanfovx"],
+            tan_fovy=cc["tanfovy"], kernel_size=float(config.kernel_size), subpixel_offset=sub, H=H, W=W, radii=radii,
+            out_color=self.image, degree=self.deg)
         ba = _C.GsrBackwardArgs()
         ba.P, ba.M, ba.R, ba.W, ba.H = P, 0, int(R), W, H
         ba.subpixel_offset = sub.data_ptr()

@@ -27,7 +27,7 @@ Anything outside the accelerated configuration (see ``supported``) runs the meth
 from __future__ import annotations
 
 import sys
-from ctypes import byref, c_int, c_size_t
+from ctypes import byref
 
 import numpy as np
 import torch
@@ -91,29 +91,15 @@ def display_composite(bg, means3D, colors, opacities, scales, rotations, viewmat
     dev = means3D.device
     P, HW = int(means3D.shape[0]), H * W
     f32 = dict(dtype=torch.float32, device=dev)
-    byte = dict(dtype=torch.uint8, device=dev)
     stream = torch.cuda.current_stream(dev).cuda_stream
     out = torch.empty(((5 if depth else 4) * HW,), **f32)       # colour [H,W,3] | accumulation [H,W] | depth [H,W]
     radii = torch.empty((P,), dtype=torch.int32, device=dev)
-    gb, ib = c_size_t(0), c_size_t(0)
-    _C._check(_lib.gsr_forward_sizes(P, 0, W, H, byref(gb), byref(ib)), "gsr_forward_sizes")
-    geom, img = torch.empty((gb.value,), **byte), torch.empty((ib.value,), **byte)
-
-    fa = _C.GsrForwardArgs()
-    fa.P, fa.D, fa.M, fa.W, fa.H = P, int(sh_degree), 0, W, H
-    fa.background, fa.means3D, fa.colors_precomp = bg.data_ptr(), means3D.data_ptr(), colors.data_ptr()
-    fa.opacities, fa.scales, fa.rotations = opacities.data_ptr(), scales.data_ptr(), rotations.data_ptr()
-    fa.scale_modifier = 1.0
-    fa.viewmatrix, fa.projmatrix, fa.campos = viewmatrix.data_ptr(), projmatrix.data_ptr(), campos.data_ptr()
-    fa.tan_fovx, fa.tan_fovy, fa.kernel_size = float(tanfovx), float(tanfovy), float(kernel_size)
-    fa.subpixel_offset = subpixel_offset.data_ptr()
-    fa.out_color, fa.radii = out.data_ptr(), radii.data_ptr()     # out_color: only checked for NULL, not written
-    R, N1 = c_int(0), c_int(0)
-    _C._check(_lib.gsr_forward_geometry(byref(fa), geom.data_ptr(), img.data_ptr(), stream, byref(R), byref(N1)),
-              "gsr_forward_geometry")
-    bb, sb = c_size_t(0), c_size_t(0)
-    _C._check(_lib.gsr_binning_sizes(P, W, H, R.value, N1.value, byref(bb), byref(sb)), "gsr_binning_sizes")
-    binning, scratch = torch.empty((bb.value,), **byte), torch.empty((sb.value,), **byte)
+    fa = _C.forward_args(background=bg, means3D=means3D, colors=colors, opacities=opacities, scales=scales,
+                         rotations=rotations, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
+                         tan_fovx=tanfovx, tan_fovy=tanfovy, kernel_size=kernel_size, subpixel_offset=subpixel_offset,
+                         H=H, W=W, radii=radii, degree=sh_degree,
+                         out_color=out)     # out_color: only checked for NULL, not written
+    geom, img, binning, scratch, R, N1 = _C._forward_geometry(fa, dev, stream)
     da = _C.GsrDisplayArgs()
     da.out_color, da.out_accum = out.data_ptr(), out[3 * HW:].data_ptr()
     dist = None
@@ -125,7 +111,7 @@ def display_composite(bg, means3D, colors, opacities, scales, rotations, viewmat
             dist = torch.empty((P,), **f32)
             da.depth_scratch = dist.data_ptr()
     _C._check(_lib.gsr_forward_display(byref(fa), byref(da), geom.data_ptr(), img.data_ptr(), binning.data_ptr(),
-                                       scratch.data_ptr(), R.value, N1.value, stream), "gsr_forward_display")
+                                       scratch.data_ptr(), R, N1, stream), "gsr_forward_display")
     # the buffers go back to torch's stream-ordered caching allocator: later allocations on this stream follow the kernels
     return out
 
