@@ -133,9 +133,10 @@ def forward(scene: dict, dtype=np.float32, tile_rows=(0, 0), stages=("preprocess
     return st
 
 
-def backward(st: dict, dL_dpix) -> dict:
+def backward(st: dict, dL_dpix, acc=None) -> dict:
     """Restated backward on the state returned by ``forward``.  Returns the 8 gradients of the reference's
-    ``rasterize_gaussians_backward`` (plus ``dL_dconic``)."""
+    ``rasterize_gaussians_backward`` (plus ``dL_dconic``).  ``acc`` ([P, 10]): run only the per-Gaussian chain rule,
+    on these accumulator rows instead of the composite's (``dL_dpix`` is then not read)."""
     dtype = st["dtype"]
     lib = _lib(dtype)
     real = c_float if dtype == np.float32 else c_double
@@ -148,13 +149,16 @@ def backward(st: dict, dL_dpix) -> dict:
         dL_dsh=np.zeros((P, M, 3), dtype), dL_dscales=np.zeros((P, 3), dtype), dL_drotations=np.zeros((P, 4), dtype))
     if P == 0:
         return out
-    dpix = _np(dL_dpix, dtype)
-    acc = np.zeros((P, 10), np.float64)
-    tr = st["tile_rows"]
-    lib.oracle_render_backward(c_int(P), c_int(W), c_int(H), c_int(tr[0]), c_int(tr[1]), _p(st["ranges"]),
-                               _p(st["point_list"]), _p(g("subpixel_offset")), _p(g("bg")), _p(st["means2D"]),
-                               _p(st["conic_opacity"]), _p(st["colors"]), _p(st["final_T"]), _p(st["n_contrib"]),
-                               _p(dpix), _p(acc))
+    if acc is None:
+        dpix = _np(dL_dpix, dtype)
+        acc = np.zeros((P, 10), np.float64)
+        tr = st["tile_rows"]
+        lib.oracle_render_backward(c_int(P), c_int(W), c_int(H), c_int(tr[0]), c_int(tr[1]), _p(st["ranges"]),
+                                   _p(st["point_list"]), _p(g("subpixel_offset")), _p(g("bg")), _p(st["means2D"]),
+                                   _p(st["conic_opacity"]), _p(st["colors"]), _p(st["final_T"]), _p(st["n_contrib"]),
+                                   _p(dpix), _p(acc))
+    else:
+        acc = np.ascontiguousarray(acc, np.float64)
     out["acc"] = acc
     shs, scales, rots = g("shs"), g("scales"), g("rotations")
     lib.oracle_preprocess_backward(

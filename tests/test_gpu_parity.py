@@ -92,16 +92,29 @@ REF_SCENES = [
 ]
 
 
-def check_grad(name, ours, ref, ref_again):
+def check_grad(name, ours, ref, ref_again, exact=None):
     """Gradient bar tied to the reference's own noise: the reference accumulates with float atomics, so two runs of
     it on the same inputs differ (`ref_noise`).  Ours must be within max(20 x that noise, 1e-5) of the tensor's largest
     magnitude -- two orders tighter than BASELINE.json's 1e-3 -- and every entry above 1e-3 of the maximum must
-    also agree RELATIVELY within 2e-3 + the noise (small-gradient Gaussians are not hidden behind the largest one)."""
+    also agree RELATIVELY within 2e-3 + the noise (small-gradient Gaussians are not hidden behind the largest one).
+
+    The run-to-run noise understates the reference's error where its atomics are biased: in the |.| channel of
+    dL/dmeans2D each pixel's term is added on its own to a sum that grows to 1e4-1e5, and terms below half an ulp of
+    it are lost, so the reference sits up to ~4e-5 of the maximum below the fp64 value while two of its runs agree to
+    ~2e-6 (measured at P=100k, 1280x720).  ``exact(name)`` (fp64 gradients of the same forward) then decides: ours
+    must be within the same bar of fp64 and closer to it than the reference."""
     ours, ref, ref_again = ours.double(), ref.double(), ref_again.double()
     scale = float(ref.abs().max()) + 1e-30
     ours_err = float((ours - ref).abs().max()) / scale
     ref_noise = float((ref_again - ref).abs().max()) / scale
-    assert ours_err <= max(20.0 * ref_noise, 1e-5), (name, ours_err, ref_noise)
+    bar = max(20.0 * ref_noise, 1e-5)
+    if ours_err > bar and exact is not None:
+        want = torch.as_tensor(np.asarray(exact(name), np.float64), device=ours.device).reshape(ours.shape)
+        ours64 = float((ours - want).abs().max()) / scale
+        ref64 = float((ref - want).abs().max()) / scale
+        assert ours64 <= bar and ours64 < ref64, (name, "to fp64: ours", ours64, "reference", ref64, "bar", bar)
+    else:
+        assert ours_err <= bar, (name, ours_err, ref_noise)
     assert ours_err < GRAD_TOL, (name, ours_err)
     big = ref.abs() > 1e-3 * scale
     if bool(big.any()):
@@ -137,10 +150,22 @@ def test_against_compiled_reference(C, dev, kw):
     assert torch.equal(v["records"][vis][:, 4:8].contiguous().view(torch.int32),
                        rv["conic_opacity"][vis].view(torch.int32))
     assert float((o["color"] - color).abs().max()) <= PIX_TOL
+    g64 = {}
+
+    def exact(n):         # fp64 gradients on the kernel's forward, computed only if a bar needs them
+        if not g64:
+            from test_adversarial_scenes import fp64_gradients
+            from oracle import cpu_oracle
+            st = cpu_oracle.forward(scene)
+            g, flips = fp64_gradients(scene, st, v["final_T"].cpu().numpy(), v["n_contrib"].cpu().numpy())
+            assert flips <= max(2, 1e-4 * v["n_contrib"].numel()), flips
+            g64.update(g)
+        return g64[n]
+
     for n in GRAD_NAMES:
         if rg[n].numel() == 0:
             continue
-        check_grad(n, o["grads"][n].view_as(rg[n]), rg[n], rg2[n])
+        check_grad(n, o["grads"][n].view_as(rg[n]), rg[n], rg2[n], exact)
 
 
 # ------------------------------------------------------------------------------------------------------
