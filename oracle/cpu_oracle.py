@@ -172,6 +172,19 @@ def backward(st: dict, dL_dpix, acc=None) -> dict:
     return out
 
 
+def pair_power(means2D, conic_opacity, g, px, py, so, dtype=np.float32) -> np.ndarray:
+    """The composite's power as oracle.c evaluates it (splat_power) for the pairs (splat g[i], pixel (px[i], py[i]),
+    sub-pixel offset so[i])."""
+    lib = _lib(dtype)
+    m, co = _np(means2D, dtype), _np(conic_opacity, dtype)
+    g = np.ascontiguousarray(np.asarray(g, np.int64).astype(np.uint32))
+    px, py = np.ascontiguousarray(px, np.int32), np.ascontiguousarray(py, np.int32)
+    s = np.ascontiguousarray(np.asarray(so).reshape(-1, 2), dtype)
+    out = np.zeros(g.size, dtype)
+    lib.oracle_pair_power(c_longlong(g.size), _p(m), _p(co), _p(g), _p(px), _p(py), _p(s), _p(out))
+    return out
+
+
 def mark_visible(means3D, viewmatrix, dtype=np.float32):
     lib = _lib(dtype)
     m, v = _np(means3D, dtype), _np(viewmatrix, dtype)

@@ -415,6 +415,23 @@ static inline real pair_power(const real* con_o, real dx, real dy) {
     return FMA(s, RL(-0.5), -u);
 }
 
+/* the reference's sample position and power of splat g at pixel (px, py) (forward.cu:340-357) */
+static inline real splat_power(const real* means2D, const real* conic_opacity, uint32_t g, int px, int py, real so_x,
+                               real so_y) {
+    const real pfx = (real)px + so_x, pfy = (real)py + so_y;
+    const real dx = means2D[2 * (size_t)g] - pfx, dy = means2D[2 * (size_t)g + 1] - pfy;
+    return pair_power(conic_opacity + 4 * (size_t)g, dx, dy);
+}
+
+/* splat_power for n (pixel, splat) pairs: splat g[i] at pixel (px[i], py[i]) with sub-pixel offset so[2 i], so[2 i + 1]
+ * (for comparison with other restatements of the composite's power, tests/test_forward_exact.py) */
+void oracle_pair_power(long long n, const real* means2D, const real* conic_opacity, const uint32_t* g,
+                       const int32_t* px, const int32_t* py, const real* so, real* out) {
+#pragma omp parallel for schedule(static)
+    for (long long i = 0; i < n; ++i)
+        out[i] = splat_power(means2D, conic_opacity, g[i], px[i], py[i], so[2 * i], so[2 * i + 1]);
+}
+
 void oracle_render(int W, int H, int ty0, int ty1, const uint32_t* ranges, const uint32_t* point_list,
                    const real* subpixel_offset, const real* means2D, const real* colors, const real* conic_opacity,
                    const real* bg, real* final_T, uint32_t* n_contrib, real* out_color) {
@@ -430,15 +447,14 @@ void oracle_render(int W, int H, int ty0, int ty1, const uint32_t* ranges, const
                     const int px = tx * TILE + lx, py = ty * TILE + ly;
                     if (px >= W || py >= H) continue;
                     const size_t pid = (size_t)W * py + px;
-                    const real pfx = (real)px + subpixel_offset[2 * pid], pfy = (real)py + subpixel_offset[2 * pid + 1];
                     real T = 1, C[3] = {0, 0, 0};
                     uint32_t contributor = 0, last = 0;
                     for (uint32_t i = r0; i < r1; ++i) {
                         contributor++;
                         const uint32_t g = point_list[i];
-                        const real dx = means2D[2 * (size_t)g] - pfx, dy = means2D[2 * (size_t)g + 1] - pfy;
                         const real* co = conic_opacity + 4 * (size_t)g;
-                        const real power = pair_power(co, dx, dy);
+                        const real power = splat_power(means2D, conic_opacity, g, px, py, subpixel_offset[2 * pid],
+                                                       subpixel_offset[2 * pid + 1]);
                         if (power > 0) continue;
                         const real alpha = R_MIN(RL(0.99), co[3] * R_EXP(power));
                         if (alpha < RL(1.0) / RL(255.0)) continue;

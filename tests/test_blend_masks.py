@@ -45,18 +45,23 @@ def _run(kw, opacity=None):
     v = _C.debug_views(geom, binning, img, P, 0, W, H, R)
     grads = _C.rasterize_gaussians_backward(*backward_args(d, radii, geom, R, binning, img))
     torch.cuda.synchronize()
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    # the mask array follows the tile ranges in the image buffer, 256-byte aligned (api.cu carve_img)
-    end = v["ranges"].data_ptr() + 8 * T
-    off = ((end + 255) // 256) * 256 - img.data_ptr()
-    masks = img.view(torch.uint8)[off:off + 4 * T * BLOCKS * WORDS].view(torch.int32).view(T, BLOCKS, WORDS)
-    out = dict(masks=masks.cpu().numpy().view(np.uint32), color=color.cpu().numpy(), radii=radii.cpu().numpy(),
+    out = dict(masks=masks_of(v, img, W, H), color=color.cpu().numpy(), radii=radii.cpu().numpy(),
                n_contrib=v["n_contrib"].cpu().numpy().astype(np.int64), ranges=v["ranges"].cpu().numpy().astype(np.int64),
                point_list=v["point_list"].cpu().numpy().astype(np.int64), records=v["records"].cpu().numpy(),
                subpixel_offset=d["subpixel_offset"].cpu().numpy(), W=W, H=H)
     for n, g in zip(GRAD_NAMES, grads):
         out["grad_" + n] = g.cpu().numpy()
     return out
+
+
+def masks_of(views, img, W, H):
+    """[T, 4, 32] blend-mask words of a forward, read from its image buffer (numpy uint32)."""
+    T = ((W + 15) // 16) * ((H + 15) // 16)
+    # the mask array follows the tile ranges in the image buffer, 256-byte aligned (api.cu carve_img)
+    end = views["ranges"].data_ptr() + 8 * T
+    off = ((end + 255) // 256) * 256 - img.data_ptr()
+    masks = img.view(torch.uint8)[off:off + 4 * T * BLOCKS * WORDS].view(torch.int32).view(T, BLOCKS, WORDS)
+    return masks.cpu().numpy().view(np.uint32)
 
 
 def _block_last(o):
