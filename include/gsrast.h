@@ -540,6 +540,40 @@ size_t gsr_uncertainty_scratch_bytes(const GsrUncertaintyArgs* args);   /* 0 for
 int gsr_uncertainty_forward(const GsrUncertaintyArgs* args, void* stream);
 int gsr_uncertainty_backward(const GsrUncertaintyArgs* args, void* stream);
 
+/* -- Uncertainty loss of every mode, in training or evaluation mode, with a capped head input (optional entry points) --
+ * The same head and `_compute_losses` (wildgaussians/method.py:339-433) for uncertainty_mode l2reg, l1reg, dino and
+ * dino+mssim (mode: GSR_UNC_MODE_*), with training = 1 (dropout2d scales in mask, BatchNorm with batch statistics and
+ * the running-statistics update, as GsrUncertaintyArgs) or 0 (BatchNorm from running_mean / running_var, which are
+ * then required and left unchanged, as is num_batches_tracked; mask is ignored).  The head runs on the head input of
+ * size uh x uw (`_scale_input`; (H, W) without a cap), padded to Hp x Wp with the input at (pad_top, pad_left); u,
+ * log u and beta are at that size.  H x W: the images gt, pred [3][H][W], ssim and msssim [H][W].
+ *   l2reg / l1reg: u is resized bilinearly to H x W when the sizes differ; loss_mult = 1 / (2 u^2) or 1 / u (not
+ *   clamped); loss = mean((1 - msssim) loss_mult) + reg_weight beta.  The 350-px fields are not read.
+ *   dino / dino+mssim: loss_mult = 1 / (2 u^2) at uh x uw, resized to the 350-px map nh x nw (the map of the image; the
+ *   caller guarantees dino_downsample gives the same grid from uh x uw), times the dino part (for dino+mssim the
+ *   smaller of it and 1 - msssim_down [nh][nw]); the loss_mult written is the resize to H x W clamped at 3.
+ *   Metrics as GsrUncertaintyArgs, from the written loss_mult.  Forward: four launches (l2reg, l1reg) or six (dino,
+ *   dino+mssim); backward four or three.  No atomics, no host synchronisation; training needs th * tw >= 2.           */
+enum { GSR_UNC_MODE_L2REG = 0, GSR_UNC_MODE_L1REG = 1, GSR_UNC_MODE_DINO = 2, GSR_UNC_MODE_DINO_MSSIM = 3 };
+typedef struct GsrUncertaintyModeArgs {
+    int mode, training;
+    int C, th, tw, Hp, Wp, pad_top, pad_left, uh, uw, H, W;
+    int nh, nw, ch, cw, nHp, nWp, npad_top, npad_left;
+    float clip_min, reg_weight, bn_eps, bn_momentum;
+    const float *feat, *feat_gt_down, *feat_pred_down, *mask;
+    const float *conv_w, *conv_b, *bn_w, *bn_b;
+    float *running_mean, *running_var;
+    long long* num_batches_tracked;
+    const float *gt, *pred, *ssim, *msssim, *msssim_down;
+    float *loss_mult, *loss, *metrics;
+    void* scratch;
+    const float* dL_dloss;
+    float *d_conv_w, *d_conv_b, *d_bn_w, *d_bn_b;
+} GsrUncertaintyModeArgs;
+size_t gsr_uncertainty_mode_scratch_bytes(const GsrUncertaintyModeArgs* args);   /* 0 for invalid sizes */
+int gsr_uncertainty_mode_forward(const GsrUncertaintyModeArgs* args, void* stream);
+int gsr_uncertainty_mode_backward(const GsrUncertaintyModeArgs* args, void* stream);
+
 /* -- Evaluation metrics (optional entry points) ------------------------------------------------------------------------
  * The per-image sums behind `compute_metrics` of wildgaussians/evaluation.py:331-352.  a, b: [B][H][W][C], each uint8
  * (a_u8 != 0, read as v / 255.0f) or fp32, contiguous, on the device; both are clipped to [0, 1] as np.clip does it.

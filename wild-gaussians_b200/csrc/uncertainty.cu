@@ -410,6 +410,372 @@ int check_args(const GsrUncertaintyArgs* a, bool backward) {
 
 unsigned blocks_for(long long n) { return (unsigned)((n + UNC_THREADS - 1) / UNC_THREADS); }
 
+// ------------------------------------------------------------------------- every mode, both BatchNorm modes, a cap
+// gsr_uncertainty_mode_*: the head runs on the (possibly capped) head input of size uh x uw; H x W is the image.  The
+// BatchNorm statistics, the cosine map and the backward's parameter kernel are the kernels above, the last called with
+// a GsrUncertaintyArgs that views the head input as the image (head_view).
+// Forward: unc_bn_stats_kernel (training) or unc_bn_eval_kernel (eval), unc_mode_head_kernel, [unc_cosine_kernel],
+// unc_mode_full_kernel, [unc_mode_down_kernel], unc_mode_finalize_kernel; [..] for dino / dino+mssim only.
+// Backward: [unc_mode_bwd_full_kernel] (l2reg / l1reg only), unc_mode_bwd_pixel_kernel, unc_mode_bwd_token_kernel,
+// unc_bwd_param_kernel.
+
+constexpr int UNC_NMODE = 7;                     // partial sums: log u (head input), then six at full resolution
+
+__host__ __device__ __forceinline__ bool dino_mode(int mode) {
+    return mode == GSR_UNC_MODE_DINO || mode == GSR_UNC_MODE_DINO_MSSIM;
+}
+
+struct ModeScratch {
+    float *mean, *invstd, *ones, *logit, *sp, *cosine, *dpart, *pfull, *pdown, *dv, *dfull, *dlogit;
+};
+
+int mode_full_blocks(const GsrUncertaintyModeArgs& a) {
+    const long long n = (long long)a.H * a.W, b = (n + UNC_THREADS - 1) / UNC_THREADS;
+    return (int)(b < UNC_MAX_BLOCKS ? b : UNC_MAX_BLOCKS);
+}
+int mode_down_blocks(const GsrUncertaintyModeArgs& a) {
+    if (!dino_mode(a.mode)) return 0;
+    const long long n = (long long)a.nh * a.nw, b = (n + UNC_THREADS - 1) / UNC_THREADS;
+    return (int)(b < UNC_MAX_BLOCKS ? b : UNC_MAX_BLOCKS);
+}
+
+size_t mode_layout(const GsrUncertaintyModeArgs& a, ModeScratch* s) {
+    const size_t T = (size_t)a.th * a.tw, C = (size_t)a.C;
+    const bool dino = dino_mode(a.mode);
+    const size_t sizes[12] = {C, C, C, T, T, dino ? (size_t)a.ch * a.cw : 0, dino ? (size_t)a.nh * a.nw : 0,
+                              (size_t)UNC_NMODE * mode_full_blocks(a), (size_t)mode_down_blocks(a), (size_t)a.uh * a.uw,
+                              dino ? 0 : (size_t)a.H * a.W, T};
+    float** dst[12] = {&s->mean, &s->invstd, &s->ones, &s->logit, &s->sp, &s->cosine, &s->dpart, &s->pfull, &s->pdown,
+                       &s->dv, &s->dfull, &s->dlogit};
+    size_t off = 0;
+    for (int i = 0; i < 12; ++i) {
+        *dst[i] = a.scratch ? (float*)a.scratch + off : nullptr;
+        off += pad64(sizes[i]);
+    }
+    return off * sizeof(float);
+}
+
+// The head input seen as the image of GsrUncertaintyArgs: what unc_bwd_param_kernel reads.
+GsrUncertaintyArgs head_view(const GsrUncertaintyModeArgs& a, const ModeScratch& s) {
+    GsrUncertaintyArgs h = {};
+    h.C = a.C; h.th = a.th; h.tw = a.tw; h.Hp = a.Hp; h.Wp = a.Wp; h.pad_top = a.pad_top; h.pad_left = a.pad_left;
+    h.H = a.uh; h.W = a.uw;
+    h.feat = a.feat; h.mask = a.training ? a.mask : s.ones;
+    h.conv_w = a.conv_w; h.conv_b = a.conv_b; h.bn_w = a.bn_w; h.bn_b = a.bn_b;
+    h.dL_dloss = a.dL_dloss; h.d_conv_w = a.d_conv_w; h.d_conv_b = a.d_conv_b; h.d_bn_w = a.d_bn_w; h.d_bn_b = a.d_bn_b;
+    return h;
+}
+
+// F.batch_norm in evaluation mode: the running statistics, no update; the channel scales are all ones.
+__global__ void __launch_bounds__(UNC_THREADS) unc_bn_eval_kernel(int C, const float* __restrict__ running_mean,
+                                                                  const float* __restrict__ running_var, float eps,
+                                                                  float* __restrict__ mean_out, float* __restrict__ invstd_out,
+                                                                  float* __restrict__ ones) {
+    const int c = blockIdx.x * UNC_THREADS + threadIdx.x;
+    if (c >= C) return;
+    mean_out[c] = running_mean[c];
+    invstd_out[c] = 1.f / sqrtf(running_var[c] + eps);
+    ones[c] = 1.f;
+}
+
+// unc_head_kernel with BatchNorm's output and the conv_seg sum over channels in double, rounded once to the logit.  In
+// evaluation mode the running statistics need not match the features, so BatchNorm's outputs can be large and the
+// channel sum cancel; the fp32 sum of unc_head_kernel then loses more than the reference's own fp32 statements do.
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_head_kernel(int C, int T, const float* __restrict__ feat,
+                                                                    const float* __restrict__ mask,
+                                                                    const float* __restrict__ mean,
+                                                                    const float* __restrict__ invstd,
+                                                                    const float* __restrict__ w, const float* __restrict__ b,
+                                                                    const float* __restrict__ gamma,
+                                                                    const float* __restrict__ beta,
+                                                                    float* __restrict__ logit, float* __restrict__ sp) {
+    extern __shared__ float prm[];                 // [5][C]: mask, mean, invstd, gamma, beta; W read from global
+    for (int c = threadIdx.x; c < C; c += UNC_THREADS) {
+        prm[c] = mask[c];
+        prm[C + c] = mean[c];
+        prm[2 * C + c] = invstd[c];
+        prm[3 * C + c] = gamma[c];
+        prm[4 * C + c] = beta[c];
+    }
+    __syncthreads();
+    const int t = blockIdx.x * UNC_THREADS + threadIdx.x;
+    if (t >= T) return;
+    double acc = 0.0;
+    for (int c = 0; c < C; ++c) {
+        const double y = ((double)feat[(size_t)c * T + t] * (double)prm[c] - (double)prm[C + c]) * (double)prm[2 * C + c] *
+                         (double)prm[3 * C + c] + (double)prm[4 * C + c];
+        acc += (double)__ldg(w + c) * y;
+    }
+    const float l = (float)(acc + (double)b[0] + 0.5413248546129181);      // log(e - 1)
+    logit[t] = l;
+    sp[t] = softplus20(l);
+}
+
+// u at head-input pixel (y, x) (clamped below; `v` unclamped).
+__device__ __forceinline__ float u_head(const GsrUncertaintyModeArgs& a, const float* __restrict__ sp, int y, int x, float& v) {
+    v = lerp2(sp, a.tw, lerp_at(a.th, a.Hp, y + a.pad_top), lerp_at(a.tw, a.Wp, x + a.pad_left));
+    return clamp_min_nan(v, a.clip_min);
+}
+
+__device__ __forceinline__ float mult_of(int mode, float u) { return mode == GSR_UNC_MODE_L1REG ? 1.f / u : inv2sq(u); }
+
+// The branch's full-resolution loss_mult at image pixel (y, x): l2reg / l1reg take it of the resized u (`uf`), the dino
+// modes resize the head input's loss_mult and clamp it at 3 (uf is then not used).
+__device__ __forceinline__ float full_mult(const GsrUncertaintyModeArgs& a, const float* __restrict__ sp, int y, int x,
+                                           float& uf) {
+    const bool dino = dino_mode(a.mode);
+    float lm, v;
+    if (a.uh == a.H && a.uw == a.W) {
+        uf = u_head(a, sp, y, x, v);
+        lm = mult_of(a.mode, uf);
+    } else {
+        const Lerp ty = lerp_at(a.uh, a.H, y), tx = lerp_at(a.uw, a.W, x);
+        float q00 = u_head(a, sp, ty.i0, tx.i0, v), q01 = u_head(a, sp, ty.i0, tx.i1, v);
+        float q10 = u_head(a, sp, ty.i1, tx.i0, v), q11 = u_head(a, sp, ty.i1, tx.i1, v);
+        if (dino) { q00 = inv2sq(q00); q01 = inv2sq(q01); q10 = inv2sq(q10); q11 = inv2sq(q11); }
+        const float r = ty.l0 * (tx.l0 * q00 + tx.l1 * q01) + ty.l1 * (tx.l0 * q10 + tx.l1 * q11);
+        uf = r;
+        lm = dino ? r : mult_of(a.mode, r);
+    }
+    return dino ? clamp_max_nan(lm, 3.f) : lm;
+}
+
+// Partials: [0] log u over the head input; over the image [1] loss_mult, [2] ssim loss_mult, [3] mse loss_mult,
+// [4] ssim, [5] msssim, [6] (1 - msssim) loss_mult (the l2reg / l1reg loss).
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_full_kernel(const GsrUncertaintyModeArgs a,
+                                                                    const float* __restrict__ sp,
+                                                                    float* __restrict__ partials) {
+    __shared__ float sh[UNC_THREADS];
+    const size_t stride = (size_t)gridDim.x * UNC_THREADS, first = blockIdx.x * (size_t)UNC_THREADS + threadIdx.x;
+    float acc[UNC_NMODE] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const size_t UHW = (size_t)a.uh * a.uw;
+    for (size_t p = first; p < UHW; p += stride) {
+        const int y = (int)(p / a.uw), x = (int)(p - (size_t)y * a.uw);
+        float v;
+        acc[0] += logf(u_head(a, sp, y, x, v));
+    }
+    const size_t HW = (size_t)a.H * a.W;
+    for (size_t p = first; p < HW; p += stride) {
+        const int y = (int)(p / a.W), x = (int)(p - (size_t)y * a.W);
+        float uf;
+        const float lm = full_mult(a, sp, y, x, uf);
+        a.loss_mult[p] = lm;
+        const float d0 = a.gt[p] - a.pred[p], d1 = a.gt[HW + p] - a.pred[HW + p], d2 = a.gt[2 * HW + p] - a.pred[2 * HW + p];
+        const float s = a.ssim[p], ms = a.msssim[p];
+        acc[1] += lm;
+        acc[2] += s * lm;
+        acc[3] += ((d0 * d0) * lm + (d1 * d1) * lm) + (d2 * d2) * lm;
+        acc[4] += s;
+        acc[5] += ms;
+        acc[6] += (1.f - ms) * lm;
+    }
+#pragma unroll
+    for (int k = 0; k < UNC_NMODE; ++k) {
+        const float r = block_sum(acc[k], sh);
+        if (threadIdx.x == 0) partials[(size_t)k * gridDim.x + blockIdx.x] = r;
+    }
+}
+
+__device__ __forceinline__ float min_nan(float x, float y) { return (x < y || x != x) ? x : y; }   // torch.min
+
+// The 350-px map: the resize of the head input's 1 / (2 u^2) times the dino part (dino+mssim: the smaller of it and
+// 1 - msssim_down).
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_down_kernel(const GsrUncertaintyModeArgs a,
+                                                                    const float* __restrict__ sp,
+                                                                    const float* __restrict__ cosine,
+                                                                    float* __restrict__ dpart, float* __restrict__ partials) {
+    __shared__ float sh[UNC_THREADS];
+    const size_t n = (size_t)a.nh * a.nw;
+    float acc = 0.f;
+    for (size_t q = blockIdx.x * (size_t)UNC_THREADS + threadIdx.x; q < n; q += (size_t)gridDim.x * UNC_THREADS) {
+        const int qy = (int)(q / a.nw), qx = (int)(q - (size_t)qy * a.nw);
+        const Lerp ty = lerp_at(a.uh, a.nh, qy), tx = lerp_at(a.uw, a.nw, qx);
+        float v;
+        const float m00 = inv2sq(u_head(a, sp, ty.i0, tx.i0, v)), m01 = inv2sq(u_head(a, sp, ty.i0, tx.i1, v));
+        const float m10 = inv2sq(u_head(a, sp, ty.i1, tx.i0, v)), m11 = inv2sq(u_head(a, sp, ty.i1, tx.i1, v));
+        const float down = ty.l0 * (tx.l0 * m00 + tx.l1 * m01) + ty.l1 * (tx.l0 * m10 + tx.l1 * m11);
+        const float cs = lerp2(cosine, a.cw, lerp_at(a.ch, a.nHp, qy + a.npad_top), lerp_at(a.cw, a.nWp, qx + a.npad_left));
+        float part = 1.f - (cs - 0.5f) / 0.5f;
+        part = part < 0.f ? 0.f : (part > 1.f ? 1.f : part);
+        if (a.mode == GSR_UNC_MODE_DINO_MSSIM) part = min_nan(part, 1.f - a.msssim_down[q]);
+        dpart[q] = part;
+        acc += part * down;
+    }
+    const float r = block_sum(acc, sh);
+    if (threadIdx.x == 0) partials[blockIdx.x] = r;
+}
+
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_finalize_kernel(const GsrUncertaintyModeArgs a, int nbf, int nbd,
+                                                                        const float* __restrict__ pfull,
+                                                                        const float* __restrict__ pdown) {
+    __shared__ double sh[UNC_THREADS];
+    double tot[UNC_NMODE + 1];
+#pragma unroll
+    for (int k = 0; k <= UNC_NMODE; ++k) {
+        const int nb = k < UNC_NMODE ? nbf : nbd;
+        const float* p = k < UNC_NMODE ? pfull + (size_t)k * nbf : pdown;
+        double s = 0.0;
+        for (int i = threadIdx.x; i < nb; i += UNC_THREADS) s += (double)p[i];
+        tot[k] = block_sum(s, sh);
+    }
+    if (threadIdx.x == 0) {
+        const double HW = (double)a.H * a.W;
+        const float beta = (float)(tot[0] / ((double)a.uh * a.uw));
+        const double mean_loss = dino_mode(a.mode) ? tot[UNC_NMODE] / ((double)a.nh * a.nw) : tot[6] / HW;
+        const float loss = (float)(mean_loss + (double)a.reg_weight * (double)beta);
+        const double mse = (double)(float)(tot[3] / tot[1]);
+        a.loss[0] = loss;
+        a.metrics[0] = loss;
+        a.metrics[1] = (float)(tot[4] / HW);
+        a.metrics[2] = (float)(tot[5] / HW);
+        a.metrics[3] = (float)(tot[2] / tot[1]);
+        a.metrics[4] = (float)mse;
+        a.metrics[5] = (float)(10.0 * log10(1.0 / mse));
+        a.metrics[6] = beta;
+    }
+}
+
+// l2reg / l1reg: dL/du of the resized u at every image pixel, g (1 - msssim) / (H W) dloss_mult/du.
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_bwd_full_kernel(const GsrUncertaintyModeArgs a,
+                                                                        const float* __restrict__ sp,
+                                                                        float* __restrict__ dfull) {
+    const size_t HW = (size_t)a.H * a.W;
+    const float g = a.dL_dloss[0] / (float)HW;
+    for (size_t p = blockIdx.x * (size_t)UNC_THREADS + threadIdx.x; p < HW; p += (size_t)gridDim.x * UNC_THREADS) {
+        const int y = (int)(p / a.W), x = (int)(p - (size_t)y * a.W);
+        float u;
+        full_mult(a, sp, y, x, u);
+        const float dm = a.mode == GSR_UNC_MODE_L1REG ? -1.f / (u * u) : -1.f / (u * (u * u));
+        dfull[p] = (g * (1.f - a.msssim[p])) * dm;
+    }
+}
+
+// sum over the outputs o of a resize in_h x in_w -> out_h x out_w of weight(o, (y, x)) src[o]: the resize's adjoint.
+__device__ __forceinline__ float resize_adjoint(int in_h, int in_w, int out_h, int out_w, int y, int x,
+                                                const float* __restrict__ src) {
+    int ylo, yhi, xlo, xhi;
+    taps_of(in_h, out_h, y, ylo, yhi);
+    taps_of(in_w, out_w, x, xlo, xhi);
+    float acc = 0.f;
+    for (int qy = ylo; qy <= yhi; ++qy) {
+        const float wy = tap_weight(in_h, out_h, qy, y);
+        if (wy == 0.f) continue;
+        float row = 0.f;
+        for (int qx = xlo; qx <= xhi; ++qx) {
+            const float wx = tap_weight(in_w, out_w, qx, x);
+            if (wx != 0.f) row += wx * src[(size_t)qy * out_w + qx];
+        }
+        acc += wy * row;
+    }
+    return acc;
+}
+
+// dL/dv at every head-input pixel (v: u before the clamp): beta's term plus the loss term through its resize's adjoint.
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_bwd_pixel_kernel(const GsrUncertaintyModeArgs a,
+                                                                         const float* __restrict__ sp,
+                                                                         const float* __restrict__ dpart,
+                                                                         const float* __restrict__ dfull,
+                                                                         float* __restrict__ dv) {
+    const size_t UHW = (size_t)a.uh * a.uw;
+    const float g = a.dL_dloss[0];
+    const float g_beta = g * a.reg_weight / (float)UHW;
+    const bool dino = dino_mode(a.mode), same = a.uh == a.H && a.uw == a.W;
+    const float g_down = dino ? g / (float)((size_t)a.nh * a.nw) : 0.f;
+    for (size_t p = blockIdx.x * (size_t)UNC_THREADS + threadIdx.x; p < UHW; p += (size_t)gridDim.x * UNC_THREADS) {
+        const int y = (int)(p / a.uw), x = (int)(p - (size_t)y * a.uw);
+        float v;
+        const float u = u_head(a, sp, y, x, v);
+        float du;
+        if (dino) {
+            const float dlm = resize_adjoint(a.uh, a.uw, a.nh, a.nw, y, x, dpart);
+            du = g_beta / u - (g_down * dlm) / (u * (u * u));
+        } else {
+            du = g_beta / u + (same ? dfull[p] : resize_adjoint(a.uh, a.uw, a.H, a.W, y, x, dfull));
+        }
+        dv[p] = v >= a.clip_min ? du : 0.f;
+    }
+}
+
+// unc_bwd_token_kernel on the head input with the gather summed in double: l2reg / l1reg give dL/dv two terms of
+// opposite sign (beta's and the loss's), so the fp32 gather of unc_bwd_token_kernel loses more than the reference's
+// own fp32 statements do.
+__global__ void __launch_bounds__(UNC_THREADS) unc_mode_bwd_token_kernel(const GsrUncertaintyModeArgs a,
+                                                                         const float* __restrict__ logit,
+                                                                         const float* __restrict__ dv,
+                                                                         float* __restrict__ dlogit) {
+    const int T = a.th * a.tw;
+    const int t = blockIdx.x * UNC_THREADS + threadIdx.x;
+    if (t >= T) return;
+    const int ty = t / a.tw, tx = t - ty * a.tw;
+    int rlo, rhi, clo, chi;
+    taps_of(a.th, a.Hp, ty, rlo, rhi);
+    taps_of(a.tw, a.Wp, tx, clo, chi);
+    rlo = max(rlo, a.pad_top); rhi = min(rhi, a.pad_top + a.uh - 1);       // the crop: only head-input pixels
+    clo = max(clo, a.pad_left); chi = min(chi, a.pad_left + a.uw - 1);
+    double acc = 0.0;
+    for (int r = rlo; r <= rhi; ++r) {
+        const float wy = tap_weight(a.th, a.Hp, r, ty);
+        if (wy == 0.f) continue;
+        const float* row = dv + (size_t)(r - a.pad_top) * a.uw - a.pad_left;
+        double s = 0.0;
+        for (int c = clo; c <= chi; ++c) {
+            const float wx = tap_weight(a.tw, a.Wp, c, tx);
+            if (wx != 0.f) s += (double)wx * (double)row[c];
+        }
+        acc += (double)wy * s;
+    }
+    const float l = logit[t];
+    const double z = exp((double)l);
+    dlogit[t] = (float)(l > 20.f ? acc : acc * z / (z + 1.0));
+}
+
+int check_mode_args(const GsrUncertaintyModeArgs* a, bool backward) {
+    if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
+    if (a->mode < GSR_UNC_MODE_L2REG || a->mode > GSR_UNC_MODE_DINO_MSSIM) {
+        set_error("bad mode %d (0..3: l2reg, l1reg, dino, dino+mssim)", a->mode);
+        return GSR_E_INVALID;
+    }
+    if (a->training != 0 && a->training != 1) { set_error("training must be 0 or 1"); return GSR_E_INVALID; }
+    if (a->C <= 0 || a->C > UNC_MAX_C) { set_error("bad channel count C=%d (1..%d)", a->C, UNC_MAX_C); return GSR_E_INVALID; }
+    const bool dino = dino_mode(a->mode);
+    const int dims[14] = {a->th, a->tw, a->Hp, a->Wp, a->uh, a->uw, a->H, a->W,
+                          dino ? a->nh : 1, dino ? a->nw : 1, dino ? a->ch : 1, dino ? a->cw : 1, dino ? a->nHp : 1,
+                          dino ? a->nWp : 1};
+    for (int d : dims)
+        if (d <= 0) { set_error("bad sizes: every size must be positive"); return GSR_E_INVALID; }
+    if (a->training && (long long)a->th * a->tw < 2) {
+        set_error("bad sizes: batch statistics need more than one token");
+        return GSR_E_INVALID;
+    }
+    if (a->th > a->Hp || a->tw > a->Wp || (dino && (a->ch > a->nHp || a->cw > a->nWp))) {
+        set_error("bad sizes: a token grid is larger than its padded image");
+        return GSR_E_INVALID;
+    }
+    if (a->pad_top < 0 || a->pad_left < 0 || a->pad_top + a->uh > a->Hp || a->pad_left + a->uw > a->Wp ||
+        (dino && (a->npad_top < 0 || a->npad_left < 0 || a->npad_top + a->nh > a->nHp || a->npad_left + a->nw > a->nWp))) {
+        set_error("bad sizes: the crop does not fit in the padded image");
+        return GSR_E_INVALID;
+    }
+    if ((long long)a->Hp * a->Wp >= (1ll << 31) || (long long)a->H * a->W >= (1ll << 31) ||
+        (dino && (long long)a->nHp * a->nWp >= (1ll << 31))) {
+        set_error("image too large");
+        return GSR_E_INVALID;
+    }
+    if (!(a->clip_min > 0.f)) { set_error("clip_min must be positive"); return GSR_E_INVALID; }
+    if (!a->feat || !a->conv_w || !a->conv_b || !a->bn_w || !a->bn_b || !a->gt || !a->pred || !a->ssim || !a->msssim ||
+        !a->loss_mult || !a->loss || !a->metrics || !a->scratch || (a->training && !a->mask) ||
+        (!a->training && (!a->running_mean || !a->running_var)) || (dino && (!a->feat_gt_down || !a->feat_pred_down)) ||
+        (a->mode == GSR_UNC_MODE_DINO_MSSIM && !a->msssim_down)) {
+        set_error("a required pointer is NULL");
+        return GSR_E_INVALID;
+    }
+    if (backward && (!a->dL_dloss || !a->d_conv_w || !a->d_conv_b || !a->d_bn_w || !a->d_bn_b)) {
+        set_error("a gradient pointer is NULL");
+        return GSR_E_INVALID;
+    }
+    return 0;
+}
+
 }  // namespace
 }  // namespace gsr
 
@@ -457,6 +823,69 @@ extern "C" int gsr_uncertainty_backward(const GsrUncertaintyArgs* a, void* strea
     unc_bwd_token_kernel<<<blocks_for(T), UNC_THREADS, 0, st>>>(*a, s.logit, s.dv, s.dlogit);
     unc_bwd_param_kernel<<<a->C, UNC_THREADS, 0, st>>>(*a, s.mean, s.invstd, s.dlogit);
     count_launches(3);
+    GSR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" size_t gsr_uncertainty_mode_scratch_bytes(const GsrUncertaintyModeArgs* a) {
+    using namespace gsr;
+    if (!a) return 0;
+    GsrUncertaintyModeArgs c = *a;
+    c.scratch = nullptr;
+    const bool dino = dino_mode(c.mode);
+    if (c.mode < GSR_UNC_MODE_L2REG || c.mode > GSR_UNC_MODE_DINO_MSSIM || c.C <= 0 || c.C > UNC_MAX_C || c.th <= 0 ||
+        c.tw <= 0 || c.uh <= 0 || c.uw <= 0 || c.H <= 0 || c.W <= 0 || (long long)c.H * c.W >= (1ll << 31) ||
+        (dino && (c.nh <= 0 || c.nw <= 0 || c.ch <= 0 || c.cw <= 0)))
+        return 0;
+    ModeScratch s;
+    return mode_layout(c, &s);
+}
+
+extern "C" int gsr_uncertainty_mode_forward(const GsrUncertaintyModeArgs* a, void* stream) {
+    using namespace gsr;
+    if (int rc = check_mode_args(a, false)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    ModeScratch s;
+    mode_layout(*a, &s);
+    const bool dino = dino_mode(a->mode);
+    const int T = a->th * a->tw, nbf = mode_full_blocks(*a), nbd = mode_down_blocks(*a);
+    if (a->training)
+        unc_bn_stats_kernel<<<a->C, UNC_THREADS, 0, st>>>(T, a->feat, a->mask, a->bn_eps, a->bn_momentum, s.mean, s.invstd,
+                                                          a->running_mean, a->running_var, a->num_batches_tracked);
+    else
+        unc_bn_eval_kernel<<<blocks_for(a->C), UNC_THREADS, 0, st>>>(a->C, a->running_mean, a->running_var, a->bn_eps,
+                                                                     s.mean, s.invstd, s.ones);
+    unc_mode_head_kernel<<<blocks_for(T), UNC_THREADS, 5 * a->C * sizeof(float), st>>>(
+        a->C, T, a->feat, a->training ? a->mask : s.ones, s.mean, s.invstd, a->conv_w, a->conv_b, a->bn_w, a->bn_b, s.logit,
+        s.sp);
+    if (dino) {
+        const int CT = a->ch * a->cw;
+        unc_cosine_kernel<<<(CT + UNC_THREADS / 32 - 1) / (UNC_THREADS / 32), UNC_THREADS, 0, st>>>(
+            a->C, CT, a->feat_gt_down, a->feat_pred_down, s.cosine);
+    }
+    unc_mode_full_kernel<<<nbf, UNC_THREADS, 0, st>>>(*a, s.sp, s.pfull);
+    if (dino) unc_mode_down_kernel<<<nbd, UNC_THREADS, 0, st>>>(*a, s.sp, s.cosine, s.dpart, s.pdown);
+    unc_mode_finalize_kernel<<<1, UNC_THREADS, 0, st>>>(*a, nbf, nbd, s.pfull, s.pdown);
+    count_launches(dino ? 6 : 4);
+    GSR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int gsr_uncertainty_mode_backward(const GsrUncertaintyModeArgs* a, void* stream) {
+    using namespace gsr;
+    if (int rc = check_mode_args(a, true)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    ModeScratch s;
+    mode_layout(*a, &s);
+    const bool dino = dino_mode(a->mode);
+    const int T = a->th * a->tw;
+    const GsrUncertaintyArgs h = head_view(*a, s);
+    if (!dino) unc_mode_bwd_full_kernel<<<mode_full_blocks(*a), UNC_THREADS, 0, st>>>(*a, s.sp, s.dfull);
+    unc_mode_bwd_pixel_kernel<<<blocks_for((long long)a->uh * a->uw), UNC_THREADS, 0, st>>>(*a, s.sp, s.dpart, s.dfull,
+                                                                                           s.dv);
+    unc_mode_bwd_token_kernel<<<blocks_for(T), UNC_THREADS, 0, st>>>(*a, s.logit, s.dv, s.dlogit);
+    unc_bwd_param_kernel<<<a->C, UNC_THREADS, 0, st>>>(h, s.mean, s.invstd, s.dlogit);
+    count_launches(dino ? 3 : 4);
     GSR_CUDA(cudaGetLastError());
     return 0;
 }

@@ -96,6 +96,19 @@ class GsrUncertaintyArgs(Structure):      # include/gsrast.h
                                          "d_bn_w", "d_bn_b")])
 
 
+class GsrUncertaintyModeArgs(Structure):      # include/gsrast.h
+    _fields_ = ([(n, c_int) for n in ("mode", "training", "C", "th", "tw", "Hp", "Wp", "pad_top", "pad_left", "uh", "uw",
+                                      "H", "W", "nh", "nw", "ch", "cw", "nHp", "nWp", "npad_top", "npad_left")] +
+                [(n, c_float) for n in ("clip_min", "reg_weight", "bn_eps", "bn_momentum")] +
+                [(n, c_void_p) for n in ("feat", "feat_gt_down", "feat_pred_down", "mask", "conv_w", "conv_b", "bn_w", "bn_b",
+                                         "running_mean", "running_var", "num_batches_tracked", "gt", "pred", "ssim", "msssim",
+                                         "msssim_down", "loss_mult", "loss", "metrics", "scratch", "dL_dloss", "d_conv_w",
+                                         "d_conv_b", "d_bn_w", "d_bn_b")])
+
+
+UNC_MODES = {"l2reg": 0, "l1reg": 1, "dino": 2, "dino+mssim": 3}       # GSR_UNC_MODE_*
+
+
 class GsrTrainLossArgs(Structure):      # include/gsrast.h
     _fields_ = ([("H", c_int), ("W", c_int), ("c_l1", c_float), ("c_ssim", c_float)] +
                 [(n, c_void_p) for n in ("toned", "raw", "gt", "mask", "weight", "grad_scale", "raw_scaled", "ssim_map",
@@ -211,6 +224,12 @@ def _load():
     lib.gsr_uncertainty_forward.restype = c_int
     lib.gsr_uncertainty_backward.argtypes = [POINTER(GsrUncertaintyArgs), c_void_p]
     lib.gsr_uncertainty_backward.restype = c_int
+    lib.gsr_uncertainty_mode_scratch_bytes.argtypes = [POINTER(GsrUncertaintyModeArgs)]
+    lib.gsr_uncertainty_mode_scratch_bytes.restype = c_size_t
+    lib.gsr_uncertainty_mode_forward.argtypes = [POINTER(GsrUncertaintyModeArgs), c_void_p]
+    lib.gsr_uncertainty_mode_forward.restype = c_int
+    lib.gsr_uncertainty_mode_backward.argtypes = [POINTER(GsrUncertaintyModeArgs), c_void_p]
+    lib.gsr_uncertainty_mode_backward.restype = c_int
     lib.gsr_train_loss_scratch_bytes.argtypes = []
     lib.gsr_train_loss_scratch_bytes.restype = c_size_t
     lib.gsr_train_loss_forward.argtypes = [POINTER(GsrTrainLossArgs), c_void_p]

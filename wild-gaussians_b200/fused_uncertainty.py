@@ -70,8 +70,22 @@ def _unsupported_model(model) -> str | None:
 
 def _unsupported(model, gt, prediction) -> str | None:
     why = _unsupported_model(model)
+    if why is None:
+        why = _unsupported_inputs(model, gt, prediction)
     if why is not None:
         return why
+    p = int(model.patch_size)
+    H, W = gt.shape[2:]
+    if -(-H // p) * -(-W // p) < 2:
+        return "needs more than one token (the reference's BatchNorm raises)"
+    if max(H, W) >= 2 ** 15:
+        return "image too large"
+    return None
+
+
+def _unsupported_inputs(model, gt, prediction) -> str | None:
+    """What the kernels need of the images and the head's parameters: fp32 [1, 3, H, W] images on one CUDA device, a
+    1 x 1 ``conv_seg`` with at most 2048 input channels, contiguous fp32 parameters and statistics beside the images."""
     bn, conv = model.bn, model.conv_seg
     if not (isinstance(gt, torch.Tensor) and isinstance(prediction, torch.Tensor)):
         return "expects tensors"
@@ -89,12 +103,6 @@ def _unsupported(model, gt, prediction) -> str | None:
         return "expects contiguous fp32 head parameters on the images' device"
     if bn.num_batches_tracked.dtype != torch.int64:
         return "expects an int64 num_batches_tracked"
-    p = int(model.patch_size)
-    H, W = gt.shape[2:]
-    if -(-H // p) * -(-W // p) < 2:
-        return "needs more than one token (the reference's BatchNorm raises)"
-    if max(H, W) >= 2 ** 15:
-        return "image too large"
     return None
 
 

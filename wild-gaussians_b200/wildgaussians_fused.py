@@ -25,7 +25,8 @@ into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (meth
 ``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
 after the last block asked for, fused attention), and ``enable(model, uncertainty=True)`` the uncertainty model's
 ``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits),
-and ``enable(model, densify=True)`` ``densify_and_prune`` and ``reset_opacity`` through ``fused_densify`` (one gather kernel
+``enable(model, uncertainty_modes=True)`` also the other modes, evaluation-mode calls and a capped head input through
+``fused_uncertainty_modes``, and ``enable(model, densify=True)`` ``densify_and_prune`` and ``reset_opacity`` through ``fused_densify`` (one gather kernel
 into final-size tensors, a GPU quantile without torch's 2^24-element limit, one synchronisation).  ``enable_method(method)`` does what ``enable`` does for
 ``method.model`` and routes ``method.optimize_embedding`` (test-time appearance optimisation, method.py:1755-1830)
 through ``fused_embedding``; ``enable_method(method, train=True)`` also routes ``method.train_iteration``
@@ -287,11 +288,21 @@ def dino_get_intermediate_layers(self, x, n=1, reshape=False, return_class_token
 def uncertainty_compute_losses(self, gt, prediction, prefix='', _cache_entry=None):
     """Drop-in for ``UncertaintyModel._compute_losses`` (method.py:363-433): ``fused_uncertainty`` where it supports the
     call (``dino`` mode, batch 1, fp32 on the GPU, training mode, no cross-process BatchNorm), the class's own method
-    otherwise."""
+    otherwise; with the model marked by ``enable(..., uncertainty_modes=True)``, ``fused_uncertainty_modes`` where that
+    supports the call (the other modes, evaluation mode, a capped head input)."""
     import fused_uncertainty
     if fused_uncertainty.supported(self, gt, prediction):
         return fused_uncertainty.compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
+    if self.__dict__.get(_MODES_MARK):
+        import fused_uncertainty_modes
+        if fused_uncertainty_modes.supported(self, gt, prediction):
+            return fused_uncertainty_modes.compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
     return type(self)._compute_losses(self, gt, prediction, prefix, _cache_entry=_cache_entry)
+
+
+# Set on an uncertainty model by enable(..., uncertainty_modes=True): its hook also takes the calls fused_uncertainty
+# refuses for the mode, evaluation mode or uncertainty_dino_max_size (fused_uncertainty_modes).
+_MODES_MARK = "_fused_uncertainty_modes"
 
 
 def densify_and_prune(self, max_grad, min_opacity, extent, enable_size_pruning, skyradius=None):
@@ -309,7 +320,7 @@ def reset_opacity(self):
 
 
 def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False,
-           uncertainty: bool = False, densify: bool = False):
+           uncertainty: bool = False, densify: bool = False, uncertainty_modes: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -321,7 +332,10 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``.
     With ``uncertainty``, ``model.uncertainty_model._compute_losses`` (reached from ``get_loss``) is rebound, as an
     instance attribute, to ``uncertainty_compute_losses``: the fused head and ``dino``-mode loss with a feature cache
-    that hits.  With ``densify``, ``model.densify_and_prune`` and ``model.reset_opacity`` are rebound, as instance
+    that hits.  With ``uncertainty_modes``, the same hook is installed and the uncertainty model marked, so that the hook
+    also routes the calls ``fused_uncertainty`` refuses only for their ``uncertainty_mode`` (``l2reg``, ``l1reg``,
+    ``dino+mssim``), evaluation mode (``optimize_embedding``'s ``get_loss(gt, gt)``) or ``uncertainty_dino_max_size``
+    through ``fused_uncertainty_modes``.  With ``densify``, ``model.densify_and_prune`` and ``model.reset_opacity`` are rebound, as instance
     attributes, to the ``fused_densify`` kernels (same results, one synchronisation per densification, any number of
     Gaussians)."""
     model._render_internal = types.MethodType(render_internal, model)
@@ -344,8 +358,10 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     if dino and backbone is not None and "get_intermediate_layers" not in backbone.__dict__:
         backbone.get_intermediate_layers = types.MethodType(dino_get_intermediate_layers, backbone)
     um = getattr(model, "uncertainty_model", None)
-    if uncertainty and um is not None and "_compute_losses" not in um.__dict__:
+    if (uncertainty or uncertainty_modes) and um is not None and "_compute_losses" not in um.__dict__:
         um._compute_losses = types.MethodType(uncertainty_compute_losses, um)
+    if uncertainty_modes and um is not None:
+        um.__dict__[_MODES_MARK] = True
     if densify:
         model.densify_and_prune = types.MethodType(densify_and_prune, model)
         model.reset_opacity = types.MethodType(reset_opacity, model)
@@ -367,6 +383,7 @@ def disable(model):
     um = getattr(model, "uncertainty_model", None)
     if um is not None:
         um.__dict__.pop("_compute_losses", None)
+        um.__dict__.pop(_MODES_MARK, None)
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
     m = sys.modules.get(type(model).__module__)
@@ -440,8 +457,8 @@ def enable_method(method, train: bool = False, render: bool = False, **kw):
     """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
     ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged.  With
     ``train``, ``method.train_iteration`` is rebound (instance attribute) to ``fused_train.train_iteration``: its loss
-    always runs as the fused op, while the backbone, ``msssim``, the uncertainty head and densification (``densify``)
-    follow their own flags.  With ``render``, ``method.render`` (every evaluation image, video frame and viewer frame) is
+    always runs as the fused op, while the backbone, ``msssim``, the uncertainty head (``uncertainty``,
+    ``uncertainty_modes``) and densification (``densify``) follow their own flags.  With ``render``, ``method.render`` (every evaluation image, video frame and viewer frame) is
     rebound (instance attribute) to ``fused_render.render``: one colour pass, one display composite and one
     device-to-host copy into pinned memory, the same result arrays."""
     enable(method.model, **kw)
