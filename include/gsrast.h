@@ -506,6 +506,39 @@ int gsr_ssim_down_forward(int B, int H, int W, int h, int w, const float* img1, 
 size_t gsr_attention_scratch_bytes(int B, int N, int H);            /* 0 for invalid sizes */
 int gsr_attention_forward(int B, int N, int H, const float* qkv, float* out, void* scratch, void* stream);
 
+/* -- Token-wise layers of the DINOv2 backbone (optional entry points, forward only) ------------------------------------
+ * The rest of `get_intermediate_layers` (wildgaussians/dinov2.py:704-813) around gsr_attention_forward, fp32 in and
+ * out with 3xTF32 tensor-core products (two accumulators per 32-wide K chunk, summed in fp32), LayerNorm statistics in
+ * double, exact-erf GELU.  Every array is contiguous on the device; those marked (16) must be 16-byte aligned.  One
+ * launch per call, no atomics (two calls are bitwise identical), no scratch, no host synchronisation.
+ *
+ * gsr_vit_tokens: `prepare_tokens_with_masks` without masks.  x: [B][3][H][W], H and W multiples of the (even) patch
+ *   size p; weight (16): the patch convolution's [C][3][p][p]; bias (16): [C]; cls: [C]; reg: [R][C] (NULL when R = 0);
+ *   pos (16): the interpolated position embedding [1 + P][C] (P = H / p * W / p); tokens (16): [B][T][C] out,
+ *   T = 1 + R + P, in the reference's order: class token + pos[0], the R register tokens, patch p + pos[1 + p].
+ *   C a multiple of 64 up to 1024, B <= 65535, B * T < 2^31.
+ * gsr_vit_linear: out = epilogue(prologue(x) weight^T + bias) for x [M][K] (16), weight [N][K] (16) (an nn.Linear's
+ *   weight as it is), bias [N] (16), out [M][N] (16); K a multiple of 4, N of 64, both up to 4096.
+ *   GSR_VIT_LN_BIAS   LayerNorm(x; ln_w, ln_b, eps) first          (norm1 + qkv)
+ *   GSR_VIT_LN_GELU   LayerNorm first, gelu_erf after the bias       (norm2 + fc1 + act)
+ *   GSR_VIT_RESIDUAL  out = resid + (x weight^T + bias) * gamma      (proj + ls1, fc2 + ls2); gamma [N] (16) or NULL
+ *                     (LayerScale is Identity), resid [M][N] (16); out may be resid (updated in place).
+ * gsr_vit_output: the final `norm` of one taken block's tokens [B][T][C] (norm_w and norm_b [C], or both NULL for
+ *   norm=False: a copy).  The patch tokens go to `patches` as [B][P][C] (GSR_VIT_LAYOUT_TOKENS) or [B][C][P], which is
+ *   reshape=True's [B][C][H / p][W / p] (GSR_VIT_LAYOUT_CHANNELS); the class token to cls [B][C] unless it is NULL.
+ *   C a multiple of 32 up to 1024, T >= R + 2, B <= 65535.                                                                 */
+#define GSR_VIT_LN_BIAS 0
+#define GSR_VIT_LN_GELU 1
+#define GSR_VIT_RESIDUAL 2
+#define GSR_VIT_LAYOUT_TOKENS 0
+#define GSR_VIT_LAYOUT_CHANNELS 1
+int gsr_vit_tokens(int B, int H, int W, int C, int patch, int R, const float* x, const float* weight, const float* bias,
+                   const float* cls, const float* reg, const float* pos, float* tokens, void* stream);
+int gsr_vit_linear(int op, int M, int K, int N, const float* x, const float* ln_w, const float* ln_b, float eps,
+                   const float* weight, const float* bias, const float* gamma, const float* resid, float* out, void* stream);
+int gsr_vit_output(int B, int T, int C, int R, int layout, const float* tokens, const float* norm_w, const float* norm_b,
+                   float eps, float* patches, float* cls, void* stream);
+
 /* -- Head and `dino`-mode loss of the uncertainty model (optional entry points) -----------------------------------------
  * After the frozen backbone: `_forward_uncertainty_features` (wildgaussians/method.py:300-323; dropout2d, BatchNorm in
  * training mode, the 1x1 conv_seg, + log(e - 1), softplus, bilinear upsample, clamp, crop) and the `dino` branch of

@@ -44,16 +44,6 @@ constexpr size_t ATT_SMEM = (size_t)ATT_STAGES * ATT_TILE_BYTES + (size_t)ATT_WG
                             2 * ATT_STAGES * sizeof(uint64_t);
 constexpr int SPLIT_THREADS = 256;
 
-__device__ __forceinline__ float4 hi4(float4 v, float4& lo) {
-    uint32_t h[4], l[4];
-    wg::split_tf32(v.x, h[0], l[0]);
-    wg::split_tf32(v.y, h[1], l[1]);
-    wg::split_tf32(v.z, h[2], l[2]);
-    wg::split_tf32(v.w, h[3], l[3]);
-    lo = make_float4(__uint_as_float(l[0]), __uint_as_float(l[1]), __uint_as_float(l[2]), __uint_as_float(l[3]));
-    return make_float4(__uint_as_float(h[0]), __uint_as_float(h[1]), __uint_as_float(h[2]), __uint_as_float(h[3]));
-}
-
 // grid (T, H, B): one 80 KB image per (key tile, head, batch) at img + ((b * H + h) * T + tile) * ATT_TILE
 __global__ void __launch_bounds__(SPLIT_THREADS) attention_split_kernel(int N, int H, int T, const float* __restrict__ qkv,
                                                                         float* __restrict__ img) {
@@ -68,7 +58,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS) attention_split_kernel(int N, i
         const int key = i % ATT_BN, u = i / ATT_BN, n = key0 + key;
         const float4 v = n < N ? *reinterpret_cast<const float4*>(kb + (size_t)n * row_stride + 4 * u) : make_float4(0, 0, 0, 0);
         float4 lo;
-        const float4 hi = hi4(v, lo);
+        const float4 hi = wg::split_tf32x4(v, lo);
         *reinterpret_cast<float4*>(dst + (u * ATT_BN + key) * 4) = hi;
         *reinterpret_cast<float4*>(dst + ATT_PART + (u * ATT_BN + key) * 4) = lo;
     }
@@ -83,8 +73,8 @@ __global__ void __launch_bounds__(SPLIT_THREADS) attention_split_kernel(int N, i
             e[s] = n < N ? vb[(size_t)n * row_stride + dim] : 0.f;
         }
         float4 rest, lo;
-        const float4 hi = hi4(make_float4(e[0], e[1], e[2], e[3]), rest);
-        const float4 mid = hi4(make_float4(e[0] - hi.x, e[1] - hi.y, e[2] - hi.z, e[3] - hi.w), lo);   // exact
+        const float4 hi = wg::split_tf32x4(make_float4(e[0], e[1], e[2], e[3]), rest);
+        const float4 mid = wg::split_tf32x4(make_float4(e[0] - hi.x, e[1] - hi.y, e[2] - hi.z, e[3] - hi.w), lo);   // exact
         *reinterpret_cast<float4*>(dst + 2 * ATT_PART + (q * ATT_D + dim) * 4) = hi;
         *reinterpret_cast<float4*>(dst + 3 * ATT_PART + (q * ATT_D + dim) * 4) = mid;
         *reinterpret_cast<float4*>(dst + 4 * ATT_PART + (q * ATT_D + dim) * 4) = lo;
@@ -142,7 +132,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(int N, in
             float4 v = row < N ? *reinterpret_cast<const float4*>(qb + (size_t)row * row_stride + 4 * u) : make_float4(0, 0, 0, 0);
             v = make_float4(v.x * 0.125f, v.y * 0.125f, v.z * 0.125f, v.w * 0.125f);
             float4 lo;
-            const float4 hi = hi4(v, lo);
+            const float4 hi = wg::split_tf32x4(v, lo);
             *reinterpret_cast<float4*>(qs + (u * 64 + r) * 4) = hi;
             *reinterpret_cast<float4*>(qs + ATT_PART + (u * 64 + r) * 4) = lo;
         }

@@ -1,5 +1,5 @@
 // wgmma.cuh -- thin inline-PTX layer over Hopper's warpgroup tensor-core instructions (wgmma), mbarriers and 1-D bulk
-// asynchronous copies, as used by appearance.cu and attention.cu.  sm_90a only.
+// asynchronous copies, as used by appearance.cu, attention.cu and vit.cu.  sm_90a only.
 //
 // Operand storage convention ("rows16"): a bf16 matrix X[ROWS][COLS] lives in shared memory as
 //     byte address(row, col) = (col / 8) * (ROWS * 16) + row * 16 + (col % 8) * 2
@@ -146,6 +146,16 @@ __device__ __forceinline__ uint32_t to_tf32(float x) {
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
     hi = to_tf32(x);
     lo = to_tf32(x - __uint_as_float(hi));
+}
+// the same for four values: returns the hi parts, lo receives the lo parts (as floats)
+__device__ __forceinline__ float4 split_tf32x4(float4 v, float4& lo) {
+    uint32_t h[4], l[4];
+    split_tf32(v.x, h[0], l[0]);
+    split_tf32(v.y, h[1], l[1]);
+    split_tf32(v.z, h[2], l[2]);
+    split_tf32(v.w, h[3], l[3]);
+    lo = make_float4(__uint_as_float(l[0]), __uint_as_float(l[1]), __uint_as_float(l[2]), __uint_as_float(l[3]));
+    return make_float4(__uint_as_float(h[0]), __uint_as_float(h[1]), __uint_as_float(h[2]), __uint_as_float(h[3]));
 }
 
 }  // namespace wg

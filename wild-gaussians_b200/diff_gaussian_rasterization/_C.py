@@ -218,6 +218,12 @@ def _load():
     lib.gsr_attention_scratch_bytes.restype = c_size_t
     lib.gsr_attention_forward.argtypes = [c_int] * 3 + [c_void_p] * 4
     lib.gsr_attention_forward.restype = c_int
+    lib.gsr_vit_tokens.argtypes = [c_int] * 6 + [c_void_p] * 8
+    lib.gsr_vit_tokens.restype = c_int
+    lib.gsr_vit_linear.argtypes = [c_int] * 4 + [c_void_p] * 3 + [c_float] + [c_void_p] * 6
+    lib.gsr_vit_linear.restype = c_int
+    lib.gsr_vit_output.argtypes = [c_int] * 5 + [c_void_p] * 3 + [c_float] + [c_void_p] * 3
+    lib.gsr_vit_output.restype = c_int
     lib.gsr_uncertainty_scratch_bytes.argtypes = [POINTER(GsrUncertaintyArgs)]
     lib.gsr_uncertainty_scratch_bytes.restype = c_size_t
     lib.gsr_uncertainty_forward.argtypes = [POINTER(GsrUncertaintyArgs), c_void_p]

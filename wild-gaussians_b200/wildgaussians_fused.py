@@ -23,7 +23,7 @@ rebinds ``model._render_internal`` to ``render_internal`` below, which returns t
 into one kernel.  ``enable(model, ssim=True)`` also routes the loss's SSIM (method.py:644-673) through ``fused_ssim``,
 ``enable(model, msssim=True)`` the uncertainty loss's ``msssim`` and ``ssim_down`` (method.py:126-187), and
 ``enable(model, dino=True)`` the uncertainty backbone's ``get_intermediate_layers`` through ``fused_dino`` (early exit
-after the last block asked for, fused attention), and ``enable(model, uncertainty=True)`` the uncertainty model's
+after the last block asked for, fused attention; ``dino_blocks=True`` also its token-wise layers), and ``enable(model, uncertainty=True)`` the uncertainty model's
 ``_compute_losses`` through ``fused_uncertainty`` (the head and the ``dino``-mode loss as kernels, a feature cache that hits),
 ``enable(model, uncertainty_modes=True)`` also the other modes, evaluation-mode calls and a capped head input through
 ``fused_uncertainty_modes``, and ``enable(model, densify=True)`` ``densify_and_prune`` and ``reset_opacity`` through ``fused_densify`` (one gather kernel
@@ -285,6 +285,17 @@ def dino_get_intermediate_layers(self, x, n=1, reshape=False, return_class_token
     return type(self).get_intermediate_layers(self, x, n, reshape, return_class_token, norm)
 
 
+def dino_blocks_get_intermediate_layers(self, x, n=1, reshape=False, return_class_token=False, norm=True):
+    """Drop-in for ``DinoVisionTransformer.get_intermediate_layers``: ``fused_dino`` with every layer on the project's
+    kernels (``blocks=True``) where it supports the backbone and input and measured faster for the token count
+    (``fused_dino.blocks_preferred``), else ``fused_dino``'s fused attention alone, else the class's own method."""
+    import fused_dino
+    for blocks in ((True, False) if fused_dino.blocks_preferred(self, x) else (False,)):
+        if fused_dino.supported(self, x, n, blocks=blocks):
+            return fused_dino.get_intermediate_layers(self, x, n, reshape, return_class_token, norm, blocks=blocks)
+    return type(self).get_intermediate_layers(self, x, n, reshape, return_class_token, norm)
+
+
 def uncertainty_compute_losses(self, gt, prediction, prefix='', _cache_entry=None):
     """Drop-in for ``UncertaintyModel._compute_losses`` (method.py:363-433): ``fused_uncertainty`` where it supports the
     call (``dino`` mode, batch 1, fp32 on the GPU, training mode, no cross-process BatchNorm), the class's own method
@@ -320,7 +331,7 @@ def reset_opacity(self):
 
 
 def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False,
-           uncertainty: bool = False, densify: bool = False, uncertainty_modes: bool = False):
+           uncertainty: bool = False, densify: bool = False, uncertainty_modes: bool = False, dino_blocks: bool = False):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -330,6 +341,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     and ``fused_ssim.ssim_down`` for supported input.  Those names are shared by every model of the module; ``disable``
     restores the originals.  With ``dino``, ``model.uncertainty_model.backbone.get_intermediate_layers`` (every DINOv2
     call of the uncertainty loss, method.py:260) is rebound, as an instance attribute, to ``dino_get_intermediate_layers``.
+    With ``dino_blocks``, it is rebound to ``dino_blocks_get_intermediate_layers`` instead, which also runs the
+    token-wise layers (patch embedding, LayerNorms, Linears, GELU, LayerScale, residuals, final norm) as kernels; it
+    replaces a ``dino`` hook, and a later ``dino`` does not downgrade it.
     With ``uncertainty``, ``model.uncertainty_model._compute_losses`` (reached from ``get_loss``) is rebound, as an
     instance attribute, to ``uncertainty_compute_losses``: the fused head and ``dino``-mode loss with a feature cache
     that hits.  With ``uncertainty_modes``, the same hook is installed and the uncertainty model marked, so that the hook
@@ -357,6 +371,10 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     backbone = _dino_backbone(model)
     if dino and backbone is not None and "get_intermediate_layers" not in backbone.__dict__:
         backbone.get_intermediate_layers = types.MethodType(dino_get_intermediate_layers, backbone)
+    if dino_blocks and backbone is not None:
+        cur = backbone.__dict__.get("get_intermediate_layers")
+        if cur is None or getattr(cur, "__func__", None) is dino_get_intermediate_layers:
+            backbone.get_intermediate_layers = types.MethodType(dino_blocks_get_intermediate_layers, backbone)
     um = getattr(model, "uncertainty_model", None)
     if (uncertainty or uncertainty_modes) and um is not None and "_compute_losses" not in um.__dict__:
         um._compute_losses = types.MethodType(uncertainty_compute_losses, um)
