@@ -143,6 +143,14 @@ typedef struct GsrBackwardArgs {
     float* dL_dsh;                /* [P,M,3]; required iff shs != NULL                      */
     float* dL_dscale;             /* [P,3];  required iff scales != NULL                    */
     float* dL_drot;               /* [P,4];  required iff rotations != NULL                 */
+    /* Fixed-order reductions: with deterministic != 0, gsr_backward / _partials and gsr_backward_colors give bitwise
+     * identical results from run to run on the same device model.  Each (tile, Gaussian) pair's sums are stored to a slot
+     * of its own, and each Gaussian adds its slots in the order of its tiles, instead of adding into the accumulator in
+     * arrival order.  Needs det_scratch (contents arbitrary) and det_marks (ALL-ZERO on entry, left all-zero), sized by
+     * gsr_backward_deterministic_sizes for this R.  The multi-GPU entry points (_peers, _marked) reject it.           */
+    int    deterministic;
+    void*  det_scratch;
+    void*  det_marks;
 } GsrBackwardArgs;
 
 /* Counters of the last forward on this geom buffer (device->host copied on request).     */
@@ -203,6 +211,8 @@ int gsr_forward_display(const GsrForwardArgs* args, const GsrDisplayArgs* displa
 
 /* -- backward ---------------------------------------------------------------------------- */
 size_t gsr_backward_scratch_bytes(int P);
+/* scratch_bytes: 48 B per instance + 4 B per Gaussian + scan temporaries; mark_bytes: 4 bits per instance.          */
+int    gsr_backward_deterministic_sizes(int P, int R, size_t* scratch_bytes, size_t* mark_bytes);
 int    gsr_backward(const GsrBackwardArgs* args, void* stream);
 /* The two halves of gsr_backward(), for the tile-row sharded (multi-GPU) path where the
  * per-Gaussian partial sums of all shards are added (NCCL all-reduce over accum_scratch, a dense
@@ -298,10 +308,16 @@ typedef struct GsrAppearanceArgs {
     float* dL_dmeans3D;               /* [P,3]  through the view direction of the SH evaluation                        */
     float* grad_pack;                 /* packed weight-gradient image                                                  */
     int*   status;                    /* optional                                                                      */
+    /* deterministic != 0: the backward entry points add the per-CTA weight-gradient partials in CTA order (one row
+     * of det_scratch per CTA, gsr_appearance_deterministic_scratch_bytes() bytes) instead of with float atomics, so the
+     * gradients are bitwise identical from run to run on the same device model.                                       */
+    int    deterministic;
+    float* det_scratch;
 } GsrAppearanceArgs;
 
 size_t gsr_appearance_packed_weight_bytes(void);
 size_t gsr_appearance_grad_pack_bytes(void);
+size_t gsr_appearance_deterministic_scratch_bytes(void);
 int gsr_appearance_pack_weights(const float* W1, const float* b1, const float* W2, const float* b2, const float* W3,
                                 const float* b3, const float* appearance_embedding, void* packed_weights, void* stream);
 int gsr_appearance_colors_forward(const GsrAppearanceArgs* args, void* stream);

@@ -135,6 +135,23 @@ size_t carve_bin_scratch(char* base, size_t N1, int W, int H, BinScratch* out) {
     return (size_t)(cur - base) + 256;
 }
 
+size_t carve_det(char* base, int P, size_t R, DetSlots* out, uint32_t** scan_tmp) {
+    DetSlots d{};
+    char* cur = base;
+    const size_t n = (size_t)(P > 0 ? P : 0);
+    uint32_t* b;
+    uint32_t* tmp;
+    take(cur, b, n + 1);
+    take(cur, tmp, scan_tmp_elems(n));
+    take(cur, d.rec, 3 * R);
+    d.base = b;
+    if (out) *out = d;
+    if (scan_tmp) *scan_tmp = tmp;
+    return (size_t)(cur - base) + 256;
+}
+
+size_t det_mark_bytes(size_t R) { return ((R * DetSlots::KB + 31) / 32) * sizeof(uint32_t); }
+
 static int check_fwd_args(const GsrForwardArgs* a) {
     if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
     if (a->P < 0 || a->W <= 0 || a->H <= 0) { set_error("bad sizes P=%d W=%d H=%d", a->P, a->W, a->H); return GSR_E_INVALID; }
@@ -445,6 +462,13 @@ int gsr_forward_display(const GsrForwardArgs* a, const GsrDisplayArgs* d, void* 
 
 size_t gsr_backward_scratch_bytes(int P) { return (size_t)(P > 0 ? P : 0) * sizeof(BwdAccum) + 256; }
 
+int gsr_backward_deterministic_sizes(int P, int R, size_t* scratch_bytes, size_t* mark_bytes) {
+    if (P < 0 || R < 0) { set_error("bad sizes"); return GSR_E_INVALID; }
+    if (scratch_bytes) *scratch_bytes = carve_det(nullptr, P, (size_t)R, nullptr, nullptr);
+    if (mark_bytes) *mark_bytes = det_mark_bytes((size_t)R);
+    return 0;
+}
+
 static int check_bwd_args(const GsrBackwardArgs* a, bool need_pix, bool need_outputs) {
     if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
     if (a->P < 0 || a->W <= 0 || a->H <= 0 || a->R < 0) { set_error("bad sizes"); return GSR_E_INVALID; }
@@ -464,6 +488,16 @@ static int check_bwd_args(const GsrBackwardArgs* a, bool need_pix, bool need_out
         if (!a->scales && !a->cov3D_precomp) { set_error("neither scales nor cov3D_precomp"); return GSR_E_INVALID; }
     }
     return 0;
+}
+
+// slots of the deterministic reductions, with base = exclusive scan of tiles_touched enqueued on s
+static int det_slots_of(const GsrBackwardArgs* a, const GeomState& g, cudaStream_t s, DetSlots* det) {
+    if (!a->det_scratch || !a->det_marks) { set_error("deterministic: det_scratch / det_marks is NULL"); return GSR_E_INVALID; }
+    uint32_t* tmp;
+    carve_det((char*)a->det_scratch, a->P, (size_t)a->R, det, &tmp);
+    det->rect = g.rect;
+    det->marks = reinterpret_cast<uint32_t*>(a->det_marks);
+    return exclusive_scan_u32(g.tiles_touched, const_cast<uint32_t*>(det->base), (size_t)a->P, tmp, s);
 }
 
 static BwdAccum* accum_of(const GsrBackwardArgs* a) {
@@ -487,14 +521,29 @@ static int backward_partials_impl(const GsrBackwardArgs* a, void* stream, const 
     int ty0, ty1;
     shard_rows(a->H, a->tile_y0, a->tile_y1, &ty0, &ty1);
     BwdAccum* accum = accum_of(a);
+    const bool det = a->deterministic != 0;
+    if (det && (peer || touched)) {
+        set_error("the multi-GPU backward reductions have no deterministic form");
+        return GSR_E_INVALID;
+    }
     // with peer accumulators the caller zeroes them (all ranks, then a barrier) before any rank adds into them
     if (!peer && !a->accum_is_zero) GSR_CUDA(cudaMemsetAsync(accum, 0, (size_t)a->P * sizeof(BwdAccum), s));
     const float* colors = a->colors_precomp ? a->colors_precomp : g.rgb;
     if (a->R > 0) {
+        DetSlots slots;
+        if (det) {
+            rc = det_slots_of(a, g, s, &slots);
+            if (rc) return rc;
+        }
         prof_begin(ST_RENDER_BWD, s);
-        rc = launch_render_bwd(*a, g, b, im, colors, accum, ty0, ty1, s, peer, touched);
+        rc = launch_render_bwd(*a, g, b, im, colors, accum, ty0, ty1, s, peer, touched, det ? &slots : nullptr);
         if (rc) return rc;
         GSR_STAGE(s, dbg, "render_bwd_packed_kernel");
+        if (det) {
+            rc = launch_det_gather_accum(a->P, g, slots, accum, s);
+            if (rc) return rc;
+            GSR_STAGE(s, dbg, "det_gather_accum_kernel");
+        }
         prof_end(ST_RENDER_BWD, s);
     }
     return 0;
@@ -582,7 +631,8 @@ int gsr_backward_colors(const GsrBackwardArgs* a, void* stream) {
         return GSR_E_INVALID;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    GSR_CUDA(cudaMemsetAsync(a->dL_dcolor, 0, (size_t)a->P * 3 * sizeof(float), s));
+    const bool det = a->deterministic != 0 && a->R > 0;     // the gather writes every row of dL_dcolor
+    if (!det) GSR_CUDA(cudaMemsetAsync(a->dL_dcolor, 0, (size_t)a->P * 3 * sizeof(float), s));
     if (a->R == 0) return 0;
     GeomState g;
     ImgState im;
@@ -592,9 +642,20 @@ int gsr_backward_colors(const GsrBackwardArgs* a, void* stream) {
     carve_bin((char*)a->binning_buffer, (size_t)a->R, &b);
     int ty0, ty1;
     shard_rows(a->H, a->tile_y0, a->tile_y1, &ty0, &ty1);
-    int rc = launch_render_color_grad(*a, g, b, im, ty0, ty1, s);
+    DetSlots slots;
+    int rc = 0;
+    if (det) {
+        rc = det_slots_of(a, g, s, &slots);
+        if (rc) return rc;
+    }
+    rc = launch_render_color_grad(*a, g, b, im, ty0, ty1, s, det ? &slots : nullptr);
     if (rc) return rc;
     GSR_STAGE(s, a->debug != 0, "render_color_grad_kernel");
+    if (det) {
+        rc = launch_det_gather_color(a->P, g, slots, a->dL_dcolor, s);
+        if (rc) return rc;
+        GSR_STAGE(s, a->debug != 0, "det_gather_color_kernel");
+    }
     return 0;
 }
 

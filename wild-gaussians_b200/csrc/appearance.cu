@@ -75,6 +75,7 @@ struct ApParams {
     float* g_gemb;          // [P,24]
     float* g_means;         // [P,3]
     float* g_pack;          // [GPACK_FLOATS] zero-initialised
+    float* det_rows;        // deterministic variants: one row per CTA (GPACK_FLOATS, or AP_H for the embedding backward)
     int* status;            // device flag: != 0 if a barrier wait timed out
 };
 
@@ -385,16 +386,32 @@ constexpr int DX_LD = 36;                                 // fp32 row stride of 
 constexpr uint32_t BDX_BYTES = AP_TILE * DX_LD * 4;       // 18432
 constexpr uint32_t BWD_SMEM = BLOB_BYTES + BX_BYTES + 2 * ACT_BYTES + BDZ_BYTES + BDO_BYTES + REST_BYTES + OUT_BYTES + BDX_BYTES + 128;
 
-// red.global.add.v2 of a weight-gradient accumulator fragment into the fp32 image `g` (row stride ld)
-template <int R>
+// red.global.add.v2 of a weight-gradient accumulator fragment into the fp32 image `g` (row stride ld); DET: plain stores
+// into the CTA's own image (the fragments of the 256 threads cover every entry)
+template <bool DET, int R>
 __device__ __forceinline__ void flush_frag(const float (&d)[R], float* g, int ld, Frag f) {
 #pragma unroll
     for (int j = 0; j < R / 4; ++j) {
         float* a = g + (size_t)f.r0 * ld + 8 * j + 2 * f.c;
         float* b = a + (size_t)8 * ld;
-        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(a), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
-        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(b), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+        if (DET) {
+            *reinterpret_cast<float2*>(a) = make_float2(d[4 * j], d[4 * j + 1]);
+            *reinterpret_cast<float2*>(b) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        } else {
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(a), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(b), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+        }
     }
+}
+
+// Deterministic variants: out[i * stride] = sum of rows[r][i] over the CTAs r in order (their images, written above)
+__global__ void __launch_bounds__(256) ap_rows_sum_kernel(const float* __restrict__ rows, int n_rows, int width,
+                                                          float* __restrict__ out, int stride) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= width) return;
+    float a = 0.f;
+    for (int r = 0; r < n_rows; ++r) a += rows[(size_t)r * width + i];
+    out[(size_t)i * stride] = a;
 }
 
 // 256 threads = two warpgroups.  Data-gradient GEMMs (M = Gaussians): warpgroup w takes rows 64 w .. 64 w + 63 of the tile.
@@ -402,7 +419,11 @@ __device__ __forceinline__ void flush_frag(const float (&d)[R], float* g, int ld
 // image, whose accumulators stay in registers across all tiles of the CTA (dW2p 72 + dW1p 16 + dW3pT 8 per thread) and
 // are reduced to HBM once per CTA.  Per-row work that cannot be split (input row, colour stage, dX) is done by thread
 // t < 128.  One CTA per SM (209 KB of shared memory).
+// DET: the deterministic variant (GsrAppearanceArgs.deterministic): db3 from per-warp partials in warp order, and each CTA
+// stores its whole gradient image to its row of det_rows for ap_rows_sum_kernel.
 constexpr int BWD_THREADS = 2 * AP_TILE;
+constexpr uint32_t BWD_SMEM_DET = BWD_SMEM + 128;         // + s_db3w [4 warps][8]
+template <bool DET>
 __global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __grid_constant__ ApParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* s_blob = smem;
@@ -416,6 +437,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __
     float* s_dx = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(s_out) + OUT_BYTES);
     uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_dx) + BDX_BYTES);
     float* s_db3 = reinterpret_cast<float*>(bars + 4);       // [8]
+    float* s_db3w = s_db3 + 8;                               // DET: [4][8] per-warp partials of warpgroup 0
     const int tid = threadIdx.x, t = tid & (AP_TILE - 1), w = tid >> 7, lane = tid & 31;
     const bool h0 = w == 0;
     const Frag f = frag_of(tid);
@@ -551,11 +573,15 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __
                 float v = dOut[j];
 #pragma unroll
                 for (int s = 16; s > 0; s >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, s);
-                if (lane == 0) atomicAdd(&s_db3[j], v);
+                if (lane == 0) {
+                    if (DET) s_db3w[(tid >> 5) * 8 + j] = v;
+                    else atomicAdd(&s_db3[j], v);
+                }
             }
         }
         fence_async_smem();
         __syncthreads();
+        if (DET && tid < AP_NOUT) s_db3[tid] += ((s_db3w[tid] + s_db3w[8 + tid]) + s_db3w[16 + tid]) + s_db3w[24 + tid];
         // coalesced copy-out of the tile's features_rest gradients (they replaced the features in s_rest)
         for (int i = tid; i < rows * AP_NREST; i += BWD_THREADS) p.g_rest[(size_t)row0 * AP_NREST + i] = s_rest[i];
         // ---- layer 3 backward --------------------------------------------------------------------------------------
@@ -618,11 +644,17 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) appearance_bwd_kernel(const __
     }
 
     // ---- reduce the CTA's weight-gradient accumulators to HBM ---------------------------------------------------------
-    if (iter > 0 && !dead) {
+    if (DET) {     // every CTA writes its whole row, zero where it had no tile
+        float* g = p.det_rows + (size_t)blockIdx.x * GPACK_FLOATS;
+        flush_frag<true>(gw2, g + GW2P, AP_K2, f);
+        flush_frag<true>(gw1, g + GW1P, AP_K1, f);
+        flush_frag<true>(gw3, g + GW3P, AP_N3, f);
+        if (tid < 16) g[GB3 + tid] = tid < AP_NOUT ? s_db3[tid] : 0.f;
+    } else if (iter > 0 && !dead) {
         float* g = p.g_pack;
-        flush_frag(gw2, g + GW2P, AP_K2, f);
-        flush_frag(gw1, g + GW1P, AP_K1, f);
-        flush_frag(gw3, g + GW3P, AP_N3, f);
+        flush_frag<false>(gw2, g + GW2P, AP_K2, f);
+        flush_frag<false>(gw1, g + GW1P, AP_K1, f);
+        flush_frag<false>(gw3, g + GW3P, AP_N3, f);
         if (tid < AP_NOUT) atomicAdd(g + GB3 + tid, s_db3[tid]);
     }
 }
@@ -696,6 +728,8 @@ __device__ __forceinline__ void toned_dout(int deg, const RowIn& in, const float
     }
 }
 
+// DET: each CTA stores its column sums to its row of det_rows (AP_H floats) for ap_rows_sum_kernel.
+template <bool DET>
 __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_emb_bwd_kernel(const __grid_constant__ ApParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* s_blob = smem;
@@ -830,7 +864,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 2) appearance_emb_bwd_kernel(cons
         __syncthreads();
     }
     // db1 slot of the gradient image: dW1p[n][AP_ONE1] = sum over the Gaussians of dZ1[:, n] (X[:, AP_ONE1] = 1)
-    if (tid < AP_H && !dead && blockIdx.x < p.num_tiles) atomicAdd(p.g_pack + GW1P + (size_t)tid * AP_K1 + AP_ONE1, colsum);
+    if (DET) {
+        if (tid < AP_H) p.det_rows[(size_t)blockIdx.x * AP_H + tid] = colsum;
+    } else if (tid < AP_H && !dead && blockIdx.x < p.num_tiles) {
+        atomicAdd(p.g_pack + GW1P + (size_t)tid * AP_K1 + AP_ONE1, colsum);
+    }
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------
@@ -876,7 +914,7 @@ static ApParams ap_params(const GsrAppearanceArgs* a) {
     p.raw = a->colors_raw; p.toned = a->colors_toned;
     p.dL_raw = a->dL_dcolors_raw; p.dL_toned = a->dL_dcolors_toned;
     p.g_dc = a->dL_dfeatures_dc; p.g_rest = a->dL_dfeatures_rest; p.g_gemb = a->dL_dembeddings; p.g_means = a->dL_dmeans3D;
-    p.g_pack = a->grad_pack; p.status = a->status;
+    p.g_pack = a->grad_pack; p.status = a->status; p.det_rows = a->det_scratch;
     return p;
 }
 
@@ -888,6 +926,9 @@ extern "C" {
 
 size_t gsr_appearance_packed_weight_bytes(void) { return BLOB_BYTES; }
 size_t gsr_appearance_grad_pack_bytes(void) { return GPACK_FLOATS * sizeof(float); }
+// one gradient image per CTA of the backward's persistent grid (one CTA per SM); the embedding backward's rows (two CTAs
+// per SM, AP_H floats each) are smaller
+size_t gsr_appearance_deterministic_scratch_bytes(void) { return (size_t)ap_num_sms() * GPACK_FLOATS * sizeof(float); }
 
 int gsr_appearance_pack_weights(const float* W1, const float* b1, const float* W2, const float* b2, const float* W3,
                                 const float* b3, const float* appearance_embedding, void* packed_weights, void* stream) {
@@ -916,11 +957,19 @@ int gsr_appearance_colors_backward(const GsrAppearanceArgs* a, void* stream) {
     if (rc || a->P == 0) return rc;
     const ApParams p = ap_params(a);
     cudaStream_t s = (cudaStream_t)stream;
-    GSR_CUDA(cudaMemsetAsync(a->grad_pack, 0, GPACK_FLOATS * sizeof(float), s));
-    GSR_CUDA(cudaFuncSetAttribute(appearance_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM));
     const int grid = min(p.num_tiles, ap_num_sms());          // persistent: one CTA per SM (187 KB of shared memory)
-    appearance_bwd_kernel<<<grid, BWD_THREADS, BWD_SMEM, s>>>(p);
-    count_launches(1);
+    if (a->deterministic) {       // every entry of grad_pack is written by the row sum
+        if (!a->det_scratch) { set_error("deterministic: det_scratch is NULL"); return GSR_E_INVALID; }
+        GSR_CUDA(cudaFuncSetAttribute(appearance_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_DET));
+        appearance_bwd_kernel<true><<<grid, BWD_THREADS, BWD_SMEM_DET, s>>>(p);
+        ap_rows_sum_kernel<<<(int)((GPACK_FLOATS + 255) / 256), 256, 0, s>>>(a->det_scratch, grid, (int)GPACK_FLOATS, a->grad_pack, 1);
+        count_launches(2);
+    } else {
+        GSR_CUDA(cudaMemsetAsync(a->grad_pack, 0, GPACK_FLOATS * sizeof(float), s));
+        GSR_CUDA(cudaFuncSetAttribute(appearance_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM));
+        appearance_bwd_kernel<false><<<grid, BWD_THREADS, BWD_SMEM, s>>>(p);
+        count_launches(1);
+    }
     GSR_CUDA(cudaGetLastError());
     return 0;
 }
@@ -945,10 +994,18 @@ int gsr_appearance_embedding_backward(const GsrAppearanceArgs* a, void* stream) 
     GSR_CUDA(cudaMemsetAsync(a->grad_pack, 0, GPACK_FLOATS * sizeof(float), s));
     if (a->P == 0) return 0;
     const ApParams p = ap_params(a);
-    GSR_CUDA(cudaFuncSetAttribute(appearance_emb_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM));
     const int grid = min(p.num_tiles, 2 * ap_num_sms());      // persistent: two resident CTAs per SM, as the forward
-    appearance_emb_bwd_kernel<<<grid, FWD_THREADS, FWD_SMEM, s>>>(p);
-    count_launches(1);
+    if (a->deterministic) {
+        if (!a->det_scratch) { set_error("deterministic: det_scratch is NULL"); return GSR_E_INVALID; }
+        GSR_CUDA(cudaFuncSetAttribute(appearance_emb_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM));
+        appearance_emb_bwd_kernel<true><<<grid, FWD_THREADS, FWD_SMEM, s>>>(p);
+        ap_rows_sum_kernel<<<1, AP_H, 0, s>>>(a->det_scratch, grid, AP_H, a->grad_pack + GW1P + AP_ONE1, AP_K1);
+        count_launches(2);
+    } else {
+        GSR_CUDA(cudaFuncSetAttribute(appearance_emb_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM));
+        appearance_emb_bwd_kernel<false><<<grid, FWD_THREADS, FWD_SMEM, s>>>(p);
+        count_launches(1);
+    }
     GSR_CUDA(cudaGetLastError());
     return 0;
 }

@@ -178,11 +178,56 @@ __device__ __forceinline__ void block_sum_f64(double (&v)[N], double (*sh)[N]) {
 int run_tile_binning(const GeomState& g, int P, int W, int H, size_t R, size_t N1, const BinScratch& bs,
                      uint32_t* point_list, uint2* ranges, cudaStream_t s, bool debug);
 
+// Slots of the deterministic backward reductions (GsrBackwardArgs.deterministic; carved by api.cu).  The instances of a
+// Gaussian are exactly the tiles of its rectangle (clipped to the tile-row band), so the (tile, Gaussian) pair with tile
+// (tx, ty) owns slot base[g] + the row-major rank of the tile in rect[g], where base is the exclusive scan of
+// tiles_touched in Gaussian order: R slots, those of one Gaussian contiguous.  A composite STORES a pair's sums to its
+// slot (no float atomics) and sets its mark bit; the gather then adds each Gaussian's marked slots in rank order and
+// clears the marks, so the marks are all-zero between calls and no slot is ever zero-filled.  KB mark bits per slot:
+// one per warp of the colour-only composite, whose four warps store separately; the backward composite uses bit 0.
+struct DetSlots {
+    static constexpr int KB = 4;
+    const uint32_t* base;     // [P+1]
+    const TileRect* rect;     // [P]
+    float4* rec;              // [R][3]: 12 floats per slot
+    uint32_t* marks;          // [ceil(KB R / 32)]
+    __device__ __forceinline__ size_t slot_of(uint32_t g, int tx, int ty) const {
+        const TileRect r = rect[g];
+        return (size_t)base[g] + (size_t)(ty - r.y0) * (r.x1 - r.x0) + (size_t)(tx - r.x0);
+    }
+    __device__ __forceinline__ void mark(size_t slot, int k) const {   // integer atomics: the result is order-free
+        const size_t bit = slot * KB + k;
+        atomicOr(marks + (bit >> 5), 1u << (bit & 31));
+    }
+    // calls f(bit) for every set mark bit of slots [first, first + n), in increasing order, and clears them (neighbouring
+    // Gaussians may share a word: atomicAnd); returns whether any was set
+    template <class F>
+    __device__ __forceinline__ bool take_marked(uint32_t first, uint32_t n, F f) const {
+        const size_t b0 = (size_t)first * KB, b1 = ((size_t)first + n) * KB;
+        bool any = false;
+        for (size_t w = b0 >> 5; w <= (b1 - 1) >> 5; ++w) {
+            const size_t lo = w << 5;
+            uint32_t m = marks[w];
+            if (b0 > lo) m &= ~0u << (b0 - lo);
+            if (b1 < lo + 32) m &= (1u << (b1 - lo)) - 1u;
+            if (m == 0) continue;
+            atomicAnd(marks + w, ~m);
+            any = true;
+            for (; m; m &= m - 1) f(lo + __ffs(m) - 1);
+        }
+        return any;
+    }
+};
+size_t carve_det(char* base, int P, size_t R, DetSlots* out, uint32_t** scan_tmp);
+size_t det_mark_bytes(size_t R);
+
 int launch_render_fwd(const GsrForwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, int ty0, int ty1, cudaStream_t s);
 // colour-only backward composite (render_fwd.cu): adds sum T alpha dL/dpixel into a.dL_dcolor
 int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im, int ty0,
-                             int ty1, cudaStream_t s);
+                             int ty1, cudaStream_t s, const DetSlots* det = nullptr);
+// deterministic colour-only backward: dL_dcolor [P,3] from the slots, every row written (render_fwd.cu)
+int launch_det_gather_color(int P, const GeomState& g, const DetSlots& det, float* dL_dcolor, cudaStream_t s);
 // display composite of an inference render (render_fwd.cu): the whole image, no backward state, the epilogue of
 // GsrDisplayArgs; depth_values [P] is composited as a fourth channel when d.depth != 0
 int launch_render_display(const GsrForwardArgs& a, const GsrDisplayArgs& d, const GeomState& g, const BinState& b,
@@ -201,7 +246,9 @@ struct PeerAccum {
 };
 int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, BwdAccum* accum, int ty0, int ty1, cudaStream_t s,
-                      const PeerAccum* peer = nullptr, unsigned char* touched = nullptr);
+                      const PeerAccum* peer = nullptr, unsigned char* touched = nullptr, const DetSlots* det = nullptr);
+// deterministic backward: the slots' fixed-order sums into the (zero) accumulator rows (render_bwd.cu)
+int launch_det_gather_accum(int P, const GeomState& g, const DetSlots& det, BwdAccum* accum, cudaStream_t s);
 // pull-mode reduction (render_bwd marks, preprocess_bwd gathers the marked rows of the other ranks): see gsrast.h
 struct PullPeers {
     const float* const* accums;          // HOST array [n_peers] of accumulator pointers (peer-mapped device addresses)

@@ -49,6 +49,8 @@ struct RenderBwdParams {
     float* mc;             // multicast address of the same symmetric buffer, or NULL
     unsigned char* touched;   // pull-mode reduction: touched[g] = 1 for every Gaussian this rank added to, or NULL
     const uint32_t* blend_mask;   // written by the forward (common.cuh)
+    // deterministic flush (DET): each (tile, Gaussian) row is stored to its own slot of det_rec and marked in det_marks
+    DetSlots det;
 };
 
 // Stage the blend-mask words a round needs: for each warp (= 8x8 block k), the NW words from word w_lo on.  Words at or
@@ -83,11 +85,16 @@ __device__ __forceinline__ void multimem_red_add_v4(float* addr, float a, float 
     asm volatile("multimem.red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"l"(addr), "f"(a), "f"(b), "f"(c),
                  "f"(d) : "memory");
 }
-// add one Gaussian's 12-float row of sums to the accumulator(s)
-template <bool PEER>
-__device__ __forceinline__ void flush_row(const RenderBwdParams& p, size_t row, float4 A, float4 B, float4 C) {
+// add one Gaussian's 12-float row of sums to the accumulator(s); DET: store it to the slot of (tile, Gaussian) instead
+template <bool PEER, bool DET>
+__device__ __forceinline__ void flush_row(const RenderBwdParams& p, size_t row, float4 A, float4 B, float4 C, int tx, int ty) {
     const size_t off = row * RB_ACC;
-    if (PEER) {
+    if (DET) {
+        const size_t slot = p.det.slot_of((uint32_t)row, tx, ty);
+        float4* dst = p.det.rec + 3 * slot;
+        dst[0] = A; dst[1] = B; dst[2] = C;
+        p.det.mark(slot, 0);
+    } else if (PEER) {
         if (p.mc != nullptr) {
             multimem_red_add_v4(p.mc + off + 0, A.x, A.y, A.z, A.w);
             multimem_red_add_v4(p.mc + off + 4, B.x, B.y, B.z, B.w);
@@ -212,7 +219,9 @@ __device__ __forceinline__ float2 hi2(const float4 v) { return make_float2(v.z, 
 // (o = opacity*coef, (A, B, C) = conic), so the linear map is applied once per (tile, Gaussian) when the tile
 // flushes its sums instead of once per pixel pair.
 // (128, 9): at most 56 registers, so that 9 CTAs (36 warps) fit an SM, as the shared memory allows
-template <bool PEER>
+// DET: the deterministic variant (GsrBackwardArgs.deterministic): rows go to per-(tile, Gaussian) slots, which
+// det_gather_accum_kernel adds in a fixed order, instead of being added into the accumulator in arrival order.
+template <bool PEER, bool DET>
 __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_constant__ RenderBwdParams p) {
     using PM = PixelMap;
     constexpr int THREADS = PM::THREADS;   // 128
@@ -405,17 +414,46 @@ __global__ void __launch_bounds__(128, 9) render_bwd_packed_kernel(const __grid_
                 const float gx = -o * ddelx_dx * (A * a0.x + B * a0.y);
                 const float gy = -o * ddely_dy * (C * a0.y + B * a0.x);
                 const float h = -0.5f * o;
-                flush_row<PEER>(p, s_id[tid], make_float4(gx, gy, a0.z, h * a0.w), make_float4(h * a1.x, h * a1.y, a1.z, a1.w),
-                          make_float4(a2.x, a2.y, 0.f, 0.f));
+                flush_row<PEER, DET>(p, s_id[tid], make_float4(gx, gy, a0.z, h * a0.w),
+                                     make_float4(h * a1.x, h * a1.y, a1.z, a1.w), make_float4(a2.x, a2.y, 0.f, 0.f), tile_x,
+                                     tile_y);
             }
         }
     }
 }
 
+// Fixed-order reduction of the deterministic flush: Gaussian g adds its marked slots in rank order (the tiles of its
+// rectangle, row-major) into its accumulator row, which is zero on entry, and clears their marks.  Rows without a mark
+// are not written.
+__global__ void __launch_bounds__(256) det_gather_accum_kernel(int P, const uint32_t* __restrict__ tiles_touched,
+                                                               DetSlots det, float4* __restrict__ accum) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= P || tiles_touched[g] == 0) return;
+    float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0, a2 = a0;
+    const bool any = det.take_marked(det.base[g], tiles_touched[g], [&](size_t bit) {
+        const float4* r = det.rec + 3 * (bit / DetSlots::KB);
+        const float4 b0 = r[0], b1 = r[1], b2 = r[2];
+        a0.x += b0.x; a0.y += b0.y; a0.z += b0.z; a0.w += b0.w;
+        a1.x += b1.x; a1.y += b1.y; a1.z += b1.z; a1.w += b1.w;
+        a2.x += b2.x; a2.y += b2.y;
+    });
+    if (any) {
+        float4* row = accum + 3 * (size_t)g;
+        row[0] = a0; row[1] = a1; row[2] = a2;
+    }
+}
+
+int launch_det_gather_accum(int P, const GeomState& g, const DetSlots& det, BwdAccum* accum, cudaStream_t s) {
+    det_gather_accum_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, g.tiles_touched, det, reinterpret_cast<float4*>(accum));
+    count_launches(1);
+    return 0;
+}
+
 int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im,
                       const float* colors, BwdAccum* accum, int ty0, int ty1, cudaStream_t s, const PeerAccum* peer,
-                      unsigned char* touched) {
+                      unsigned char* touched, const DetSlots* det) {
     RenderBwdParams p;
+    p.det = det ? *det : DetSlots{};
     p.touched = touched;
     p.peers = peer ? (float* const*)(peer->peers) : nullptr;
     p.n_peers = peer ? peer->n_peers : 0;
@@ -429,9 +467,11 @@ int launch_render_bwd(const GsrBackwardArgs& a, const GeomState& g, const BinSta
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);
     if (peer)   // the flush adds into every rank's accumulator
-        render_bwd_packed_kernel<true><<<grid, 128, 0, s>>>(p);
+        render_bwd_packed_kernel<true, false><<<grid, 128, 0, s>>>(p);
+    else if (det)
+        render_bwd_packed_kernel<false, true><<<grid, 128, 0, s>>>(p);
     else
-        render_bwd_packed_kernel<false><<<grid, 128, 0, s>>>(p);
+        render_bwd_packed_kernel<false, false><<<grid, 128, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

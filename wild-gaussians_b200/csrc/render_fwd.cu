@@ -300,6 +300,7 @@ struct ColorGradParams {
     const uint32_t* blend_mask;
     const float* dL_dpix;      // [3,H,W]
     float* dL_dcolor;          // [P,3], zeroed before the launch
+    DetSlots det;              // DET: warp k of a tile stores its 3 sums of a Gaussian to floats 3k.. of the pair's slot
 };
 
 // sum of (v0, v1, v2) over the warp in 6 shuffles (a 4-value butterfly with one padding slot); lane l ends up holding the
@@ -315,6 +316,8 @@ __device__ __forceinline__ float butterfly3(float v0, float v1, float v2, int la
     return x;
 }
 
+// DET: the deterministic variant (GsrBackwardArgs.deterministic): det_gather_color_kernel adds the slots in a fixed order.
+template <bool DET>
 __global__ void __launch_bounds__(128) render_color_grad_kernel(const __grid_constant__ ColorGradParams p) {
     using PM = PixelMap;
     constexpr int WARPS = PM::WARPS;
@@ -431,15 +434,47 @@ __global__ void __launch_bounds__(128) render_color_grad_kernel(const __grid_con
                 T = make_float2(upd0 ? test_T.x : T.x, upd1 ? test_T.y : T.y);
                 const float2 c0 = mul2(aT, dL0), c1 = mul2(aT, dL1), c2 = mul2(aT, dL2);
                 const float v = butterfly3(c0.x + c0.y, c1.x + c1.y, c2.x + c2.y, lane);
-                if (owner) atomicAdd(p.dL_dcolor + 3 * (size_t)s_id[j] + comp, v);
+                if (DET) {
+                    if (owner) {
+                        const size_t slot = p.det.slot_of(s_id[j], tile_x, tile_y);
+                        reinterpret_cast<float*>(p.det.rec + 3 * slot)[3 * warp + comp] = v;
+                        if (comp == 0) p.det.mark(slot, warp);
+                    }
+                } else if (owner) {
+                    atomicAdd(p.dL_dcolor + 3 * (size_t)s_id[j] + comp, v);
+                }
             }
         }
     }
 }
 
+// Fixed-order gather of the deterministic colour-only backward: Gaussian g adds its marked slots in rank order and, within
+// a slot, the warps in order; every row of dL_dcolor is written (zero for a Gaussian no pixel blends).
+__global__ void __launch_bounds__(256) det_gather_color_kernel(int P, const uint32_t* __restrict__ tiles_touched, DetSlots det,
+                                                               float* __restrict__ dL_dcolor) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= P) return;
+    float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+    if (tiles_touched[g] != 0)
+        det.take_marked(det.base[g], tiles_touched[g], [&](size_t bit) {
+            const float* r = reinterpret_cast<const float*>(det.rec + 3 * (bit / DetSlots::KB)) + 3 * (bit % DetSlots::KB);
+            c0 += r[0]; c1 += r[1]; c2 += r[2];
+        });
+    dL_dcolor[3 * (size_t)g + 0] = c0;
+    dL_dcolor[3 * (size_t)g + 1] = c1;
+    dL_dcolor[3 * (size_t)g + 2] = c2;
+}
+
+int launch_det_gather_color(int P, const GeomState& g, const DetSlots& det, float* dL_dcolor, cudaStream_t s) {
+    det_gather_color_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, g.tiles_touched, det, dL_dcolor);
+    count_launches(1);
+    return 0;
+}
+
 int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const BinState& b, const ImgState& im, int ty0,
-                             int ty1, cudaStream_t s) {
+                             int ty1, cudaStream_t s, const DetSlots* det) {
     ColorGradParams p;
+    p.det = det ? *det : DetSlots{};
     p.W = a.W; p.H = a.H; p.grid_x = tiles_x(a.W); p.ty0 = ty0;
     p.ranges = im.ranges; p.point_list = b.point_list;
     p.subpixel_offset = reinterpret_cast<const float2*>(a.subpixel_offset);
@@ -447,7 +482,10 @@ int launch_render_color_grad(const GsrBackwardArgs& a, const GeomState& g, const
     p.dL_dpix = a.dL_dpix; p.dL_dcolor = a.dL_dcolor;
     if (ty1 <= ty0) return 0;
     dim3 grid(p.grid_x, ty1 - ty0, 1);
-    render_color_grad_kernel<<<grid, 128, 0, s>>>(p);
+    if (det)
+        render_color_grad_kernel<true><<<grid, 128, 0, s>>>(p);
+    else
+        render_color_grad_kernel<false><<<grid, 128, 0, s>>>(p);
     count_launches(1);
     return 0;
 }

@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import warnings
 from ctypes import POINTER, Structure, byref, c_char_p, c_float, c_int, c_size_t, c_void_p
 
 import torch
@@ -45,7 +46,7 @@ class GsrBackwardArgs(Structure):
         ("accum_scratch", c_void_p), ("accum_is_zero", c_int),
         ("dL_dmean2D", c_void_p), ("dL_dconic", c_void_p), ("dL_dopacity", c_void_p), ("dL_dcolor", c_void_p),
         ("dL_dmean3D", c_void_p), ("dL_dcov3D", c_void_p), ("dL_dsh", c_void_p), ("dL_dscale", c_void_p),
-        ("dL_drot", c_void_p),
+        ("dL_drot", c_void_p), ("deterministic", c_int), ("det_scratch", c_void_p), ("det_marks", c_void_p),
     ]
 
 
@@ -56,7 +57,7 @@ class GsrAppearanceArgs(Structure):
         ("campos", c_void_p), ("packed_weights", c_void_p), ("colors_raw", c_void_p), ("colors_toned", c_void_p),
         ("dL_dcolors_raw", c_void_p), ("dL_dcolors_toned", c_void_p), ("dL_dfeatures_dc", c_void_p),
         ("dL_dfeatures_rest", c_void_p), ("dL_dembeddings", c_void_p), ("dL_dmeans3D", c_void_p),
-        ("grad_pack", c_void_p), ("status", c_void_p),
+        ("grad_pack", c_void_p), ("status", c_void_p), ("deterministic", c_int), ("det_scratch", c_void_p),
     ]
 
 
@@ -149,6 +150,9 @@ def _load():
     lib.gsr_forward_display.restype = c_int
     lib.gsr_backward_scratch_bytes.argtypes = [c_int]
     lib.gsr_backward_scratch_bytes.restype = c_size_t
+    lib.gsr_backward_deterministic_sizes.argtypes = [c_int, c_int, POINTER(c_size_t), POINTER(c_size_t)]
+    lib.gsr_backward_deterministic_sizes.restype = c_int
+    lib.gsr_appearance_deterministic_scratch_bytes.restype = c_size_t
     lib.gsr_backward.argtypes = [POINTER(GsrBackwardArgs), c_void_p]
     lib.gsr_backward_partials.argtypes = [POINTER(GsrBackwardArgs), c_void_p]
     lib.gsr_backward_finalize.argtypes = [POINTER(GsrBackwardArgs), c_void_p]
@@ -315,6 +319,55 @@ def clear_geometry_cache() -> None:
 
 def geometry_cache_hits() -> int:
     return int(_geom_cache.get("hits", 0))
+
+
+# ---- reproducible runs under torch.use_deterministic_algorithms(True) ------------------------------------------------
+# The flag is read on every call: when it is set, the backward composite, the colour-only backward and the colour op add
+# their partial sums in a fixed order (GsrBackwardArgs / GsrAppearanceArgs.deterministic), and the paths that have no such
+# form refuse to run, as PyTorch's own ops do.
+def deterministic() -> bool:
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def refuse_nondeterministic(path: str) -> None:
+    """Under ``torch.use_deterministic_algorithms(True)`` raise ``RuntimeError`` naming ``path``, or warn when the flag
+    was set with ``warn_only=True``; nothing otherwise."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"{path} does not have a deterministic implementation, but you set "
+           "'torch.use_deterministic_algorithms(True)'. Run it on one GPU without a tile-row split across processes, "
+           "or call torch.use_deterministic_algorithms(True, warn_only=True) to run it anyway with a warning.")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
+# Mark bits of the deterministic backward: all-zero between calls (each call clears the bits it set), so one buffer is
+# kept per (device, stream) and grown with zeros; a call that failed leaves it dirty and it is re-zeroed.
+_det_marks: dict = {}
+
+
+def deterministic_buffers(P: int, R: int, dev):
+    """(scratch, marks) for a deterministic ``GsrBackwardArgs`` call with P Gaussians and R instances.  Call
+    ``deterministic_done(marks)`` after the library call returned 0."""
+    sb, mb = c_size_t(0), c_size_t(0)
+    _check(_lib.gsr_backward_deterministic_sizes(int(P), int(R), byref(sb), byref(mb)), "gsr_backward_deterministic_sizes")
+    key = (str(dev), int(_stream(dev)))
+    ent = _det_marks.get(key)
+    if ent is None or ent[0].numel() < mb.value:
+        ent = [torch.zeros((max(mb.value, 256),), dtype=torch.uint8, device=dev), "zero"]
+        _det_marks[key] = ent
+    elif ent[1] != "zero":
+        ent[0].zero_()
+    ent[1] = "dirty"
+    return torch.empty((sb.value,), dtype=torch.uint8, device=dev), ent[0]
+
+
+def deterministic_done(marks) -> None:
+    for ent in _det_marks.values():
+        if ent[0] is marks:
+            ent[1] = "zero"
 
 
 def _check(rc: int, what: str) -> None:
@@ -578,6 +631,11 @@ def _backward_impl(mode, accum, background, means3D, radii, colors, scales, rota
             a.dL_dsh = _ptr(dL_dsh)
             a.dL_dscale = dL_dscales.data_ptr() if have_scales else None
             a.dL_drot = dL_drotations.data_ptr() if have_scales else None
+        keep_det = None
+        if deterministic() and peer is None and marked is None and pull is None and mode != "finalize" and int(R) > 0:
+            keep_det = deterministic_buffers(P, int(R), dev)
+            a.deterministic = 1
+            a.det_scratch, a.det_marks = keep_det[0].data_ptr(), keep_det[1].data_ptr()
         if marked is not None:        # pull-mode first half: local sums + marks
             a.accum_is_zero = 1
             _check(_lib.gsr_backward_partials_marked(byref(a), marked.data_ptr(), _stream(dev)), "gsr_backward_partials_marked")
@@ -601,6 +659,8 @@ def _backward_impl(mode, accum, background, means3D, radii, colors, scales, rota
         if mode != "finalize":
             _accum_state[id(accum)] = "dirty"          # until a finalize has consumed (and thereby cleared) it
         _check(fn(byref(a), _stream(dev)), "gsr_backward" + ("" if mode == "both" else "_" + mode))
+        if keep_det is not None:
+            deterministic_done(keep_det[1])
         if mode != "partials":
             _accum_state[id(accum)] = "zero"
     return accum if mode == "partials" else outs

@@ -103,6 +103,9 @@ class _FusedColors(torch.autograd.Function):
             a.dL_dfeatures_dc, a.dL_dfeatures_rest = d_dc.data_ptr(), d_rest.data_ptr()
             a.dL_dembeddings, a.dL_dmeans3D = d_gemb.data_ptr(), d_means.data_ptr()
             a.grad_pack, a.status = pack.data_ptr(), status.data_ptr()
+            if _C.deterministic():            # per-CTA partials added in CTA order instead of float atomics
+                rows = torch.empty((_lib.gsr_appearance_deterministic_scratch_bytes() // 4,), **f32)
+                a.deterministic, a.det_scratch = 1, rows.data_ptr()
             _C._check(_lib.gsr_appearance_colors_backward(byref(a), _stream(dev)), "gsr_appearance_colors_backward")
             _last_status["bwd"] = status
             dW1, db1 = torch.empty((128, 59), **f32), torch.empty((128,), **f32)

@@ -175,6 +175,7 @@ class EmbeddingLoop:
         aa.colors_toned, aa.dL_dcolors_toned = self.toned_v.data_ptr(), self.dtoned_v.data_ptr()
         aa.grad_pack, aa.status = self.pack.data_ptr(), self.status.data_ptr()
         self.app_args = aa
+        self.det_rows = None                  # per-CTA rows of the deterministic embedding backward, made on first use
         self.param.grad = torch.zeros_like(self.param)
         self.metrics = torch.zeros((self.iters, 3), **f32)    # loss, mse, log10(mse)
 
@@ -206,10 +207,23 @@ class EmbeddingLoop:
     def embedding_grad(self, dL_dimage):
         """dL/d(embedding) [32] (into ``self.param.grad``) from dL/d(toned image) [3,H,W] on the current colours."""
         s = self.stream
-        self.bwd_args.dL_dpix = dL_dimage.data_ptr()
-        _C._check(_lib.gsr_backward_colors(byref(self.bwd_args), s), "gsr_backward_colors")
+        ba, aa = self.bwd_args, self.app_args
+        ba.dL_dpix = dL_dimage.data_ptr()
+        det = _C.deterministic()              # read on every call, as PyTorch's ops do
+        ba.deterministic = aa.deterministic = int(det)
+        keep = None
+        if det and ba.R > 0:
+            keep = _C.deterministic_buffers(ba.P, ba.R, self.dcolor.device)
+            ba.det_scratch, ba.det_marks = keep[0].data_ptr(), keep[1].data_ptr()
+        if det and self.det_rows is None:
+            self.det_rows = torch.empty((_lib.gsr_appearance_deterministic_scratch_bytes() // 4,), dtype=torch.float32,
+                                        device=self.dcolor.device)
+        aa.det_scratch = self.det_rows.data_ptr() if det else None
+        _C._check(_lib.gsr_backward_colors(byref(ba), s), "gsr_backward_colors")
+        if keep is not None:
+            _C.deterministic_done(keep[1])
         torch.index_select(self.dcolor, 0, self.vis, out=self.dtoned_v)
-        _C._check(_lib.gsr_appearance_embedding_backward(byref(self.app_args), s), "gsr_appearance_embedding_backward")
+        _C._check(_lib.gsr_appearance_embedding_backward(byref(aa), s), "gsr_appearance_embedding_backward")
         u = self.unpacked
         _C._check(_lib.gsr_appearance_unpack_grads(self.pack.data_ptr(), self.w[0].data_ptr(), self.param.data_ptr(),
                                                    u[0].data_ptr(), u[1].data_ptr(), u[2].data_ptr(), u[3].data_ptr(),

@@ -216,6 +216,8 @@ def reduced_partials(bwd_args, P: int, device, group=None, shard=None) -> torch.
     per-Gaussian sums (flat fp32, first P*12 entries).  Either NCCL all-reduce of the partial arrays or, with
     GSR_PEER_REDUCE, the reduction fused into the kernel through peer / multicast memory."""
     from diff_gaussian_rasterization import _C
+    _C.refuse_nondeterministic("parallel.reduced_partials (multi-GPU backward reduction: peer red, multicast or NCCL "
+                               "all-reduce)")
     H, W = int(bwd_args[14].size(1)), int(bwd_args[14].size(2))
     st = _peers(P, H, W, device, group)
     if st is not None:
@@ -236,6 +238,8 @@ def sharded_backward(bwd_args, bands, group=None):
     ``_C.rasterize_gaussians_backward`` (upstream gradient replicated); returns the 8 gradient tensors, complete on every
     rank."""
     from diff_gaussian_rasterization import _C
+    _C.refuse_nondeterministic("parallel.sharded_backward (multi-GPU backward reduction: peer red, multicast, pull or "
+                               "NCCL all-reduce)")
     rank = dist.get_rank(group)
     means3D = bwd_args[1]
     H, W = int(bwd_args[14].size(1)), int(bwd_args[14].size(2))
