@@ -496,6 +496,24 @@ int gsr_train_loss_backward(const GsrTrainLossArgs* args, void* stream);
  * NULL (not both).  One launch.                                                                                          */
 int gsr_unpack_u8(int H, int W, const unsigned char* img_hwc, const unsigned char* mask_hw, float* img_chw, float* mask_out,
                   void* stream);
+/* The inverse of gsr_unpack_u8 for training data kept on the device, with its byte-exactness check.  Each item is one
+ * fp32 image (C = 3, element (c, y, x) at src[c * stride_c + y * stride_y + x * stride_x], so the reference's [3,H,W]
+ * views of HWC arrays and contiguous CHW tensors both qualify) or mask (C = 1, stride_c unused).  It writes dst
+ * [H][W][C] uint8 with u = clip(rint(x * 255), 0, 255), rounding half to even, and ORs into *flags (device memory,
+ * cleared by the caller): GSR_PACK_NOT_EXACT when some element's (float)u / 255.0f differs from it bit for bit (NaN,
+ * +-inf, -0.0, out of range, off the k / 255 grid), GSR_PACK_NOT_BINARY when some element is neither 0 nor 1.  Up to
+ * GSR_PACK_MAX_ITEMS items per call, one launch, no host synchronisation; `items` is host memory.                      */
+#define GSR_PACK_MAX_ITEMS 32
+#define GSR_PACK_NOT_EXACT 1u
+#define GSR_PACK_NOT_BINARY 2u
+typedef struct GsrPackItem {
+    const float* src;
+    unsigned char* dst;
+    unsigned int* flags;
+    long long stride_c, stride_y, stride_x;
+    int H, W, C, reserved;
+} GsrPackItem;
+int gsr_pack_u8_exact(const GsrPackItem* items, int n, void* stream);
 
 /* -- Image-quality statistics of the uncertainty loss (optional entry points, forward only) -----------------------------
  * `msssim(x, y, max_size, min_size)` and `ssim_down(x, y, max_size)` of wildgaussians/method.py:126-187.  img1, img2:

@@ -192,6 +192,34 @@ __global__ void __launch_bounds__(TL_THREADS) unpack_u8_kernel(int HW, const uns
     if (mask_hw) mask_out[p] = (float)mask_hw[p] / 255.0f;
 }
 
+// The inverse of unpack_u8_kernel with the byte-exactness check of fused_train.as_bytes, per element x:
+//   u = clip(rint(x * 255f), 0, 255) (rintf rounds half to even, as np.rint; fmaxf sends NaN to 0),
+//   exact when the bits of (float)u / 255.0f equal the bits of x,
+// so NaN, +-inf, -0.0, values outside [0, 1] and anything off the k / 255 grid are not exact.  The bytes are written
+// whatever the verdict; the caller keeps them only for an item whose flag word stays clear of GSR_PACK_NOT_EXACT.
+struct PackBatch {
+    GsrPackItem items[GSR_PACK_MAX_ITEMS];
+};
+
+__global__ void __launch_bounds__(TL_THREADS) pack_u8_exact_kernel(PackBatch b) {
+    const GsrPackItem& it = b.items[blockIdx.y];
+    const long long HW = (long long)it.H * it.W, n = HW * it.C;
+    unsigned int f = 0u;
+    for (long long o = (long long)blockIdx.x * TL_THREADS + threadIdx.x; o < n; o += (long long)gridDim.x * TL_THREADS) {
+        const int c = it.C == 3 ? (int)(o % 3) : 0;
+        const long long p = it.C == 3 ? o / 3 : o;
+        const long long y = p / it.W, x = p - y * it.W;
+        const float v = __ldg(it.src + c * it.stride_c + y * it.stride_y + x * it.stride_x);
+        const float t = fminf(fmaxf(rintf(__fmul_rn(v, 255.f)), 0.f), 255.f);
+        const unsigned int u = (unsigned int)t;
+        it.dst[o] = (unsigned char)u;
+        if (__float_as_uint(__fdiv_rn((float)u, 255.f)) != __float_as_uint(v)) f |= GSR_PACK_NOT_EXACT;
+        if (!(v == 0.f || v == 1.f)) f |= GSR_PACK_NOT_BINARY;
+    }
+    f = __reduce_or_sync(0xffffffffu, f);
+    if ((threadIdx.x & 31) == 0 && f) atomicOr(it.flags, f);
+}
+
 static int tl_check(const GsrTrainLossArgs* a, bool backward) {
     if (!a) { set_error("args is NULL"); return GSR_E_INVALID; }
     if (a->H <= 0 || a->W <= 0 || (long long)a->H * a->W > (1ll << 31) / 3) {
@@ -260,6 +288,32 @@ extern "C" int gsr_unpack_u8(int H, int W, const unsigned char* img_hwc, const u
     const int HW = H * W;
     unpack_u8_kernel<<<(HW + TL_THREADS - 1) / TL_THREADS, TL_THREADS, 0, (cudaStream_t)stream>>>(HW, img_hwc, mask_hw,
                                                                                                   img_chw, mask_out);
+    count_launches(1);
+    GSR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int gsr_pack_u8_exact(const GsrPackItem* items, int n, void* stream) {
+    using namespace gsr;
+    if (!items) { set_error("items is NULL"); return GSR_E_INVALID; }
+    if (n < 1 || n > GSR_PACK_MAX_ITEMS) { set_error("item count %d outside [1, %d]", n, GSR_PACK_MAX_ITEMS); return GSR_E_INVALID; }
+    PackBatch b;
+    long long most = 0;
+    for (int i = 0; i < n; ++i) {
+        const GsrPackItem& it = items[i];
+        if (it.H <= 0 || it.W <= 0 || (long long)it.H * it.W > (1ll << 31) / 3) {
+            set_error("item %d: bad image size H=%d W=%d", i, it.H, it.W);
+            return GSR_E_INVALID;
+        }
+        if (it.C != 1 && it.C != 3) { set_error("item %d: C=%d is neither 1 nor 3", i, it.C); return GSR_E_INVALID; }
+        if (!it.src || !it.dst || !it.flags) { set_error("item %d: src, dst or flags is NULL", i); return GSR_E_INVALID; }
+        b.items[i] = it;
+        const long long e = (long long)it.H * it.W * it.C;
+        most = e > most ? e : most;
+    }
+    const long long blocks = (most + TL_THREADS - 1) / TL_THREADS;
+    const dim3 grid((unsigned int)(blocks < 2048 ? blocks : 2048), (unsigned int)n);
+    pack_u8_exact_kernel<<<grid, TL_THREADS, 0, (cudaStream_t)stream>>>(b);
     count_launches(1);
     GSR_CUDA(cudaGetLastError());
     return 0;

@@ -117,6 +117,15 @@ class GsrTrainLossArgs(Structure):      # include/gsrast.h
                                          "d_raw")])
 
 
+class GsrPackItem(Structure):      # include/gsrast.h
+    _fields_ = ([(n, c_void_p) for n in ("src", "dst", "flags")] +
+                [(n, ctypes.c_longlong) for n in ("stride_c", "stride_y", "stride_x")] +
+                [(n, c_int) for n in ("H", "W", "C", "reserved")])
+
+
+PACK_MAX_ITEMS, PACK_NOT_EXACT, PACK_NOT_BINARY = 32, 1, 2      # GSR_PACK_MAX_ITEMS / _NOT_EXACT / _NOT_BINARY
+
+
 class GsrMetricsArgs(Structure):      # include/gsrast.h
     _fields_ = ([(n, c_int) for n in ("B", "H", "W", "C", "a_u8", "b_u8")] + [("a", c_void_p), ("b", c_void_p)] +
                 [("taps", ctypes.c_double * 11), ("c1", ctypes.c_double), ("c2", ctypes.c_double)] +
@@ -248,6 +257,8 @@ def _load():
     lib.gsr_train_loss_backward.restype = c_int
     lib.gsr_unpack_u8.argtypes = [c_int, c_int] + [c_void_p] * 5
     lib.gsr_unpack_u8.restype = c_int
+    lib.gsr_pack_u8_exact.argtypes = [POINTER(GsrPackItem), c_int, c_void_p]
+    lib.gsr_pack_u8_exact.restype = c_int
     lib.gsr_metrics_scratch_bytes.argtypes = [c_int] * 4
     lib.gsr_metrics_scratch_bytes.restype = c_size_t
     lib.gsr_metrics_forward.argtypes = [POINTER(GsrMetricsArgs), c_void_p]

@@ -18,6 +18,16 @@ protected-iteration detach, the densification block on the model's own methods, 
   about 50 s for a 1,700-image scene).  The slot is filled once the render's kernels are queued, so the host's copy
   (about 1.5 ms at 1920x1080) overlaps the composites instead of preceding the render's first launch; at 1920x1080
   the copy outlasts the composites, so its tail is still exposed.
+* Resident ground truth (opt-in: ``enable_method(method, train=True, resident=True, resident_bytes=None)``).  At the
+  first call the cameras are taken in index order while they fit ``resident_bytes`` (None: half of the device memory
+  free then; ``plan``) and kept in device memory: uint8 HWC where byte-exact, fp32 otherwise, masks likewise.  The
+  fp32 lists go up through two alternating pinned chunks on a side stream; ``gsr_pack_u8_exact`` checks and packs each
+  chunk on the device (the predicate of ``as_bytes`` and the binary-mask test) while the next one uploads, and its
+  flags are read back once per chunk.  ``as_bytes`` never runs on a resident camera.  Per step the drawn camera is
+  unpacked from the store on the compute stream: no host fill, no copy, no event.  Cameras over the budget are staged
+  as above by a stager that serves only them.  The store is keyed like the stager and rebuilt when the lists change;
+  ``disable_method`` frees it.  The kernels and their inputs are those of the staged path, so the step computes the
+  same bits.
 * Dispatch.  ``supported`` checks every image and mask once per (image list, mask list) and then only the lists'
   identity and length, so a step's host work does not grow with the number of training images.
 * Loss.  ``train_loss`` below: scale_grads by the mask and ``loss_mult``, L1, the weighted means and every metric sum in
@@ -49,12 +59,14 @@ import torch
 
 from diff_gaussian_rasterization import _C
 
-__all__ = ["train_iteration", "supported", "train_loss", "as_bytes", "METRICS"]
+__all__ = ["train_iteration", "supported", "train_loss", "as_bytes", "pack_u8_exact", "plan", "METRICS"]
 
 _lib = _C._lib
 # the loss op's metric vector (csrc/train_loss.cu), then the step's total loss
 METRICS = ("l1_loss", "ssim", "mse", "psnr", "mask_percentage", "ssim_masked", "mse_masked", "l1_loss_masked")
 _stagers: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+_stores: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+_metrics_hosts: dict = {}
 _image_checks: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
 
 
@@ -165,13 +177,32 @@ class _Entry:
             self.mask_binary = bool(np.all((mv == 0) | (mv == 1)))
 
 
-class _Stager:
-    """Two pinned host slots and two device slots; a side stream carries the host-to-device copies."""
+def _unpack(H, W, img_u8, mask_u8, img_f32, mask_f32, has_mask, device, stream):
+    """(gt [3,H,W], mask [1,H,W] or None) as fresh fp32 tensors on `stream`, from device bytes (uint8 HWC / HW, unpacked
+    by ``gsr_unpack_u8``) or device fp32 values (copied): exactly one of img_u8 / img_f32, at most one of the masks."""
+    f32 = dict(dtype=torch.float32, device=device)
+    gt = torch.empty((3, H, W), **f32)
+    mask = torch.empty((1, H, W), **f32) if has_mask else None
+    if img_u8 is not None or mask_u8 is not None:
+        _C._check(_lib.gsr_unpack_u8(H, W, None if img_u8 is None else img_u8.data_ptr(),
+                                     None if mask_u8 is None else mask_u8.data_ptr(), gt.data_ptr(),
+                                     None if mask is None else mask.data_ptr(), stream.cuda_stream), "gsr_unpack_u8")
+    if img_f32 is not None:
+        gt.copy_(img_f32.view(3, H, W))
+    if mask_f32 is not None:
+        mask.copy_(mask_f32.view(1, H, W))
+    return gt, mask
 
-    def __init__(self, images, masks, device):
+
+class _Stager:
+    """Two pinned host slots and two device slots; a side stream carries the host-to-device copies.  ``cameras``: the
+    indices it serves (all by default; the resident store's leftovers otherwise)."""
+
+    def __init__(self, images, masks, device, cameras=None):
         self.images, self.masks = images, masks
-        self.entries = [_Entry(img, None if masks is None else masks[i]) for i, img in enumerate(images)]
-        cap = max((e.img_bytes + e.mask_bytes for e in self.entries), default=256)
+        cameras = range(len(images)) if cameras is None else cameras
+        self.entries = {i: _Entry(images[i], None if masks is None else masks[i]) for i in cameras}
+        cap = max((e.img_bytes + e.mask_bytes for e in self.entries.values()), default=256)
         self.device = device
         self.host = [torch.empty((cap,), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
         self.dev = [torch.empty((cap,), dtype=torch.uint8, device=device) for _ in range(2)]
@@ -179,7 +210,6 @@ class _Stager:
         self.consumed = [None, None]     # the compute stream is done reading the device slot
         self.stream = torch.cuda.Stream(device)
         self.turn = 0
-        self.metrics_host = torch.empty((64,), dtype=torch.float32, pin_memory=True)
 
     def upload(self, cid: int):
         e = self.entries[cid]
@@ -211,19 +241,12 @@ class _Stager:
         k, e = pending
         cur = torch.cuda.current_stream(self.device)
         cur.wait_event(self.copied[k])
-        f32 = dict(dtype=torch.float32, device=self.device)
-        d = self.dev[k]
-        gt = torch.empty((3, e.H, e.W), **f32)
-        mask = torch.empty((1, e.H, e.W), **f32) if e.mask_bytes else None
-        img_src = d[:e.H * e.W * 3].data_ptr() if e.img_u8 is not None else None
-        mask_src = d[e.img_bytes:].data_ptr() if e.mask_u8 is not None else None
-        if img_src is not None or mask_src is not None:
-            _C._check(_lib.gsr_unpack_u8(e.H, e.W, img_src, mask_src, gt.data_ptr(),
-                                         None if mask is None else mask.data_ptr(), cur.cuda_stream), "gsr_unpack_u8")
-        if e.img_f32 is not None:
-            gt.copy_(d[:12 * e.H * e.W].view(torch.float32).view(3, e.H, e.W))
-        if e.mask_f32 is not None:
-            mask.copy_(d[e.img_bytes:e.img_bytes + 4 * e.H * e.W].view(torch.float32).view(1, e.H, e.W))
+        d, HW = self.dev[k], e.H * e.W
+        gt, mask = _unpack(e.H, e.W, d if e.img_u8 is not None else None,
+                           d[e.img_bytes:] if e.mask_u8 is not None else None,
+                           d[:12 * HW].view(torch.float32) if e.img_f32 is not None else None,
+                           d[e.img_bytes:e.img_bytes + 4 * HW].view(torch.float32) if e.mask_f32 is not None else None,
+                           e.mask_bytes > 0, self.device, cur)
         self.consumed[k] = torch.cuda.Event()
         self.consumed[k].record(cur)
         return gt, mask, e.mask_binary
@@ -235,13 +258,238 @@ def _lists_key(method):
     return (id(images), None if images is None else len(images), id(masks), None if masks is None else len(masks))
 
 
-def _stager(method, device) -> _Stager:
+def _stager(method, device, cameras=None) -> _Stager:
+    """The method's stager for ``cameras`` (all when None), rebuilt when the lists or the camera set change."""
     s = _stagers.get(method)
-    key = _lists_key(method)
+    key = (_lists_key(method), None if cameras is None else tuple(cameras))
     if s is None or s.key != key or s.images is not method.train_images or s.device != device:
-        s = _stagers[method] = _Stager(method.train_images, method.train_masks, device)
+        s = _stagers[method] = _Stager(method.train_images, method.train_masks, device, cameras)
         s.key = key
     return s
+
+
+def _metrics_host(device) -> torch.Tensor:
+    """A pinned buffer for the step's metric read-back, one per device."""
+    t = _metrics_hosts.get(device)
+    if t is None:
+        t = _metrics_hosts[device] = torch.empty((64,), dtype=torch.float32, pin_memory=True)
+    return t
+
+
+# ---- resident training data ------------------------------------------------------------------------------------------
+
+# Set on a method by ``wildgaussians_fused.enable_method(method, train=True, resident=True, resident_bytes=...)``: the
+# byte budget of its device image store, or None for half of the device memory free when the store is built.
+RESIDENT_MARK = "_fused_resident_bytes"
+PACK_CHUNK_BYTES = 64 << 20      # pinned bounce chunk (two alternate); a camera larger than this gets a chunk its size
+
+
+def resident_bytes(H: int, W: int, image_exact: bool, mask: bool, mask_exact: bool) -> int:
+    """Device bytes one camera takes in the resident store: uint8 HWC for byte-exact data, fp32 otherwise."""
+    return H * W * ((3 if image_exact else 12) + ((1 if mask_exact else 4) if mask else 0))
+
+
+class _Budget:
+    """First fit in index order: a camera is taken when its bytes fit in what the cameras taken before left over."""
+
+    def __init__(self, budget: int):
+        self.left = int(budget)
+
+    def take(self, nbytes: int) -> bool:
+        if nbytes > self.left:
+            return False
+        self.left -= nbytes
+        return True
+
+
+def plan(sizes, budget) -> list:
+    """Which cameras of the per-camera byte sizes ``sizes`` the resident store keeps under ``budget`` (``_Budget``)."""
+    b = _Budget(budget)
+    return [b.take(s) for s in sizes]
+
+
+def _pack_items(items, stream):
+    """One ``gsr_pack_u8_exact`` launch over ``items``: (src fp32 tensor, its (c, y, x) element strides, C, H, W, dst
+    uint8 tensor, flags int32 tensor element)."""
+    arr = (_C.GsrPackItem * len(items))()
+    for a, (src, strides, C, H, W, dst, flag) in zip(arr, items):
+        a.src, a.dst, a.flags = src.data_ptr(), dst.data_ptr(), flag.data_ptr()
+        a.stride_c, a.stride_y, a.stride_x = strides
+        a.H, a.W, a.C = H, W, C
+    _C._check(_lib.gsr_pack_u8_exact(arr, len(items), stream.cuda_stream), "gsr_pack_u8_exact")
+
+
+def pack_u8_exact(x: torch.Tensor):
+    """The device check and pack of one fp32 CUDA image ``[3,H,W]`` (any strides) or mask ``[H,W]`` / ``[1,H,W]``:
+    ``(bytes, exact, binary)`` with ``bytes`` the uint8 ``[H,W,3]`` / ``[H,W]`` that ``gsr_unpack_u8`` turns back into
+    ``x`` when ``exact`` (the predicate of ``as_bytes``), and ``binary`` whether every element is 0 or 1.  Reads the
+    verdict back, so it synchronises; the resident store batches its launches and read-backs instead."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32):
+        raise RuntimeError("fused_train.pack_u8_exact expects an fp32 CUDA tensor")
+    if x.dim() == 3 and x.shape[0] == 3:
+        C, H, W = 3, int(x.shape[1]), int(x.shape[2])
+        strides = tuple(x.stride())
+    elif x.dim() == 2 or (x.dim() == 3 and x.shape[0] == 1):
+        C, H, W = 1, int(x.shape[-2]), int(x.shape[-1])
+        strides = (0, x.stride(-2), x.stride(-1))
+    else:
+        raise RuntimeError(f"fused_train.pack_u8_exact expects [3,H,W], [H,W] or [1,H,W], got {tuple(x.shape)}")
+    dst = torch.empty((H, W, 3) if C == 3 else (H, W), dtype=torch.uint8, device=x.device)
+    flags = torch.zeros((1,), dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        _pack_items([(x, strides, C, H, W, dst, flags[0])], torch.cuda.current_stream(x.device))
+    f = int(flags.item())
+    return dst, not f & _C.PACK_NOT_EXACT, not f & _C.PACK_NOT_BINARY
+
+
+def _host_layout(image):
+    """(pinned-view maker, device element strides) that keep ``image``'s memory order in the bounce chunk, so the
+    host's copy into pinned memory is a plain memcpy for the reference's HWC-backed [3,H,W] views."""
+    _, H, W = image.shape
+    if image.permute(1, 2, 0).is_contiguous():
+        return (lambda buf: buf.view(H, W, 3).permute(2, 0, 1)), (1, 3 * W, 3)
+    return (lambda buf: buf.view(3, H, W)), (H * W, W, 1)
+
+
+class _ResidentEntry:
+    """One camera in device memory: image as uint8 HWC or fp32 [3,H,W], mask as uint8 HW, fp32 [1,H,W] or absent."""
+    __slots__ = ("H", "W", "img", "img_u8", "mask", "mask_u8", "mask_binary")
+
+    def receive(self, device, stream):
+        m = self.mask
+        gt, mask = _unpack(self.H, self.W, self.img if self.img_u8 else None, m if m is not None and self.mask_u8 else None,
+                           None if self.img_u8 else self.img, m if m is not None and not self.mask_u8 else None,
+                           m is not None, device, stream)
+        return gt, mask, self.mask_binary
+
+
+class _Resident:
+    """The training images and masks that fit ``budget`` bytes (``_Budget``), on the device; the rest are left to a
+    ``_Stager``.  Built once: the fp32 lists go through two alternating pinned chunks on a side stream, each chunk is
+    checked and packed by one ``gsr_pack_u8_exact`` launch while the next uploads, and its flags are read back once."""
+
+    def __init__(self, images, masks, device, budget):
+        self.images, self.masks, self.device = images, masks, device
+        self.entries: dict = {}
+        budget = _Budget(budget)
+        cur = torch.cuda.current_stream(device)
+        side = torch.cuda.Stream(device)
+        sizes = []
+        for i, img in enumerate(images):
+            n = int(img.shape[1]) * int(img.shape[2])
+            sizes.append((_align(12 * n), _align(4 * n) if masks is not None else 0))
+        # a camera whose bytes could not fit even if every camera still in flight were dropped is never uploaded
+        lower = [resident_bytes(int(x.shape[1]), int(x.shape[2]), True, masks is not None, True) for x in images]
+        cap = max([PACK_CHUNK_BYTES] + [a + b for a, b in sizes])
+        host = [torch.empty((cap,), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+        dev = [torch.empty((cap,), dtype=torch.uint8, device=device) for _ in range(2)]
+        flags_host = [torch.empty((_C.PACK_MAX_ITEMS,), dtype=torch.int32, pin_memory=True) for _ in range(2)]
+        copied, consumed = [None, None], [None, None]
+        pending = None
+        batch, used = [], 0
+        k = 0
+
+        def flush():
+            nonlocal pending, batch, used, k
+            if not batch:
+                return
+            if copied[k] is not None:
+                copied[k].synchronize()                  # the pinned chunk's previous upload is done
+            hb, items = host[k], []
+            for cam in batch:
+                cid, off, moff = cam["cid"], cam["off"], cam["moff"]
+                img = images[cid]
+                H, W = int(img.shape[1]), int(img.shape[2])
+                view, strides = _host_layout(img)
+                view(hb[off:off + 12 * H * W].view(torch.float32)).copy_(img)
+                cam["strides"] = strides
+                if masks is not None:
+                    hb[moff:moff + 4 * H * W].view(torch.float32).view(H, W).copy_(masks[cid].reshape(H, W))
+            if consumed[k] is not None:
+                side.wait_event(consumed[k])             # the device chunk's previous batch is done with it
+            with torch.cuda.stream(side):
+                dev[k][:used].copy_(hb[:used], non_blocking=True)
+                copied[k] = torch.cuda.Event()
+                copied[k].record(side)
+            cur.wait_event(copied[k])
+            flags = torch.zeros((len(batch) * 2,), dtype=torch.int32, device=device)
+            for j, cam in enumerate(batch):
+                H, W, off, moff = cam["H"], cam["W"], cam["off"], cam["moff"]
+                cam["img"] = torch.empty((H, W, 3), dtype=torch.uint8, device=device)
+                items.append((dev[k][off:].view(torch.float32), cam["strides"], 3, H, W, cam["img"], flags[2 * j]))
+                if masks is not None:
+                    cam["mask"] = torch.empty((H, W), dtype=torch.uint8, device=device)
+                    items.append((dev[k][moff:].view(torch.float32), (0, W, 1), 1, H, W, cam["mask"], flags[2 * j + 1]))
+            _pack_items(items, cur)
+            fh = flags_host[k][:flags.numel()]
+            fh.copy_(flags, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(cur)
+            prev, pending = pending, (k, batch, fh, done)
+            if prev is not None:
+                finish(*prev)                            # while this chunk uploads and packs
+            batch, used, k = [], 0, k ^ 1
+
+        def finish(slot, cams, fh, done):
+            done.synchronize()
+            f = fh.tolist()
+            for j, cam in enumerate(cams):
+                H, W, off, moff = cam["H"], cam["W"], cam["off"], cam["moff"]
+                img_exact = not f[2 * j] & _C.PACK_NOT_EXACT
+                mask_exact = masks is None or not f[2 * j + 1] & _C.PACK_NOT_EXACT
+                if not budget.take(resident_bytes(H, W, img_exact, masks is not None, mask_exact)):
+                    continue
+                e = _ResidentEntry()
+                e.H, e.W, e.img_u8, e.mask_u8 = H, W, img_exact, mask_exact
+                src = dev[slot][off:off + 12 * H * W].view(torch.float32)
+                sc, sy, sx = cam["strides"]
+                e.img = cam["img"] if img_exact else src.as_strided((3, H, W), (sc, sy, sx)).clone(
+                    memory_format=torch.contiguous_format)
+                e.mask, e.mask_binary = None, True
+                if masks is not None:
+                    e.mask = cam["mask"] if mask_exact else dev[slot][moff:moff + 4 * H * W].view(torch.float32).view(
+                        1, H, W).clone()
+                    e.mask_binary = not f[2 * j + 1] & _C.PACK_NOT_BINARY
+                self.entries[cam["cid"]] = e
+            consumed[slot] = torch.cuda.Event()
+            consumed[slot].record(cur)
+
+        for cid, img in enumerate(images):
+            if lower[cid] > budget.left:
+                continue
+            a, b = sizes[cid]
+            if batch and (used + a + b > cap or 2 * len(batch) + 2 > _C.PACK_MAX_ITEMS):
+                flush()
+            H, W = int(img.shape[1]), int(img.shape[2])
+            batch.append(dict(cid=cid, H=H, W=W, off=used, moff=used + a))
+            used += a + b
+        flush()
+        if pending is not None:
+            finish(*pending)
+        self.staged = [i for i in range(len(images)) if i not in self.entries]
+
+
+def _resident(method, device):
+    """The method's resident store, or None when ``enable_method(..., resident=True)`` did not mark it."""
+    if RESIDENT_MARK not in method.__dict__:
+        return None
+    s = _stores.get(method)
+    key = _lists_key(method)
+    if s is None or s.key != key or s.images is not method.train_images or s.device != device:
+        _stores.pop(method, None)                        # free the old store before the new one is built
+        budget = method.__dict__[RESIDENT_MARK]
+        if budget is None:
+            budget = torch.cuda.mem_get_info(device)[0] // 2
+        with torch.cuda.device(device):
+            s = _stores[method] = _Resident(method.train_images, method.train_masks, device, budget)
+        s.key = key
+    return s
+
+
+def release(method) -> None:
+    """Free the method's resident store (``wildgaussians_fused.disable_method``)."""
+    if _cacheable(method):
+        _stores.pop(method, None)
 
 
 # ---- the step --------------------------------------------------------------------------------------------------------
@@ -352,15 +600,21 @@ def train_iteration(method, step):
     assert viewpoint_cam.image_sizes is not None, "Image sizes are required for training"
     image_width, image_height = viewpoint_cam.image_sizes
 
-    stager = _stager(self, device)
+    store = _resident(self, device)
+    stager = None
+    if store is None or camera_id not in store.entries:
+        stager = _stager(self, device, None if store is None else store.staged)
     embedding = model.get_embedding(train_image_id=camera_id)
     render_pkg = model._render_internal(viewpoint_cam, config=cfg, embedding=embedding, kernel_size=cfg.kernel_size)
     image_toned, image, viewspace_point_tensor, radii = (render_pkg["render"], render_pkg["raw_render"],
                                                          render_pkg["viewspace_points"], render_pkg["radii"])
     assert image.shape == (3, image_height, image_width), f"image.shape={image.shape}"
-    # the render's kernels are queued: the host fills the pinned slot and the copy travels on a side stream while they
-    # run; the compute stream waits for it here, before the first use
-    gt_image, mask, mask_binary = stager.receive(stager.upload(camera_id))
+    if stager is None:                    # resident: unpacked from device memory on the compute stream
+        gt_image, mask, mask_binary = store.entries[camera_id].receive(device, torch.cuda.current_stream(device))
+    else:
+        # the render's kernels are queued: the host fills the pinned slot and the copy travels on a side stream while
+        # they run; the compute stream waits for it here, before the first use
+        gt_image, mask, mask_binary = stager.receive(stager.upload(camera_id))
 
     uncertainty_loss = 0
     metrics: dict = {}
@@ -407,7 +661,7 @@ def train_iteration(method, step):
         parts = [loss_metrics, loss.detach().reshape(1)] + ([unc_metrics] if unc_metrics is not None else [])
         vec = torch.cat(parts)
         n = int(vec.numel())
-        host = stager.metrics_host[:n]
+        host = _metrics_host(device)[:n]
         host.copy_(vec, non_blocking=True)
         read = torch.cuda.Event()
         read.record(torch.cuda.current_stream(device))

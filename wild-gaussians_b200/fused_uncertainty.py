@@ -19,7 +19,11 @@ with the same CPU fp32 values: entries written by either path are hit by the oth
 deterministic and draws no random numbers, so a hit returns what running it again would.  The full-resolution and the
 350-px features cannot collide under one entry: when ``dino_downsample`` resizes, the 350-px image has at most 25
 patches on its longer side and the full-resolution one at least 26; when it does not, both are the same image.  Cached
-features are copied in with ``non_blocking=True`` from pageable memory.
+features are copied in with ``non_blocking=True`` from pageable memory.  On a model marked by
+``wildgaussians_fused.enable(model, resident_features=True)`` (or ``enable_method(..., resident=True)``) a new entry is
+instead a device clone owned by the cache while the cache's device entries fit its byte budget, so a hit copies
+nothing; the reference's ``_get_dino_cached`` reads such entries unchanged (``.to(x.device)`` of a device tensor is the
+tensor).  ``release_features`` moves them back to host tensors.
 
 ``supported(model, gt, prediction)`` tells which calls this covers; ``wildgaussians_fused.enable(model,
 uncertainty=True)`` routes the rest to the reference's own method.
@@ -35,11 +39,14 @@ import torch.nn.functional as F
 
 from diff_gaussian_rasterization import _C
 
-__all__ = ["compute_losses", "compute_losses_on_device", "supported"]
+__all__ = ["compute_losses", "compute_losses_on_device", "supported", "release_features"]
 
 _lib = _C._lib
 DINO_MAX_SIZE = 350                               # method.py:386-387
 METRICS = ("loss", "ssim", "msssim", "ssim_discounted", "mse_discounted", "psnr_discounted", "beta")
+# Set on an uncertainty model by enable(..., resident_features=True): [budget in bytes of the feature cache's device
+# entries], None until the first store, which takes half of the device memory then free.
+RESIDENT_MARK = "_fused_resident_features"
 
 
 def _distributed_bn(bn) -> bool:
@@ -133,8 +140,30 @@ def _features(model, x, cache_entry):
     with torch.no_grad():
         f = model.backbone.get_intermediate_layers(x, n=[model.backbone.num_heads - 1], reshape=True)[-1]
     if cache_entry is not None:
-        model._images_cache[(cache_entry, f.shape)] = f.detach().cpu()
+        model._images_cache[(cache_entry, f.shape)] = _cached(model, f)
     return f
+
+
+def _cached(model, f):
+    """What the cache stores for the features ``f``: a device clone within a marked model's budget, else a host copy."""
+    mark = model.__dict__.get(RESIDENT_MARK)
+    if mark is not None and f.is_cuda:
+        if mark[0] is None:
+            mark[0] = torch.cuda.mem_get_info(f.device)[0] // 2
+        used = sum(v.nbytes for v in model._images_cache.values() if isinstance(v, torch.Tensor) and v.is_cuda)
+        if used + f.nbytes <= mark[0]:
+            return f.detach().clone(memory_format=torch.contiguous_format)
+    return f.detach().cpu()
+
+
+def release_features(model) -> None:
+    """Unmark ``model`` and turn the device entries of its feature cache into the host tensors it would hold unmarked."""
+    model.__dict__.pop(RESIDENT_MARK, None)
+    cache = getattr(model, "_images_cache", None)
+    if cache:
+        for k, v in list(cache.items()):
+            if isinstance(v, torch.Tensor) and v.is_cuda:
+                cache[k] = v.cpu()
 
 
 class _Loss(torch.autograd.Function):

@@ -331,7 +331,8 @@ def reset_opacity(self):
 
 
 def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = False, dino: bool = False,
-           uncertainty: bool = False, densify: bool = False, uncertainty_modes: bool = False, dino_blocks: bool = False):
+           uncertainty: bool = False, densify: bool = False, uncertainty_modes: bool = False, dino_blocks: bool = False,
+           resident_features: bool = False, feature_cache_bytes: int | None = None):
     """Route this model's ``_render_internal`` and ``compute_3D_filter`` through the fused paths (instance attributes; the
     class is untouched) and, with ``optimizer``, turn its Adam into the single-kernel ``fused_adam.FusedAdam`` in place.
 
@@ -351,7 +352,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
     ``dino+mssim``), evaluation mode (``optimize_embedding``'s ``get_loss(gt, gt)``) or ``uncertainty_dino_max_size``
     through ``fused_uncertainty_modes``.  With ``densify``, ``model.densify_and_prune`` and ``model.reset_opacity`` are rebound, as instance
     attributes, to the ``fused_densify`` kernels (same results, one synchronisation per densification, any number of
-    Gaussians)."""
+    Gaussians).  With ``resident_features``, the uncertainty model's feature cache (``_images_cache``, filled by the fused
+    losses) stores new entries as device tensors while they fit ``feature_cache_bytes`` (None: half of the device memory
+    free at the first store), host tensors beyond; ``disable`` moves the device entries back to the host."""
     model._render_internal = types.MethodType(render_internal, model)
     model.compute_3D_filter = types.MethodType(compute_3D_filter, model)
     if optimizer and type(getattr(model, "optimizer", None)) is torch.optim.Adam:
@@ -380,6 +383,9 @@ def enable(model, optimizer: bool = True, ssim: bool = False, msssim: bool = Fal
         um._compute_losses = types.MethodType(uncertainty_compute_losses, um)
     if uncertainty_modes and um is not None:
         um.__dict__[_MODES_MARK] = True
+    if resident_features and um is not None:
+        import fused_uncertainty
+        um.__dict__[fused_uncertainty.RESIDENT_MARK] = [None if feature_cache_bytes is None else int(feature_cache_bytes)]
     if densify:
         model.densify_and_prune = types.MethodType(densify_and_prune, model)
         model.reset_opacity = types.MethodType(reset_opacity, model)
@@ -402,6 +408,8 @@ def disable(model):
     if um is not None:
         um.__dict__.pop("_compute_losses", None)
         um.__dict__.pop(_MODES_MARK, None)
+        if "fused_uncertainty" in sys.modules:
+            sys.modules["fused_uncertainty"].release_features(um)
     if type(getattr(model, "optimizer", None)).__name__ == "FusedAdam":
         model.optimizer.__class__ = torch.optim.Adam
     m = sys.modules.get(type(model).__module__)
@@ -471,14 +479,24 @@ def render(method, camera, options=None, **kwargs):
     return fused_render.render(method, camera, options, **kwargs)
 
 
-def enable_method(method, train: bool = False, render: bool = False, **kw):
+def enable_method(method, train: bool = False, render: bool = False, resident: bool = False,
+                  resident_bytes: int | None = None, **kw):
     """``enable(method.model, **kw)`` and ``method.optimize_embedding`` rebound (instance attribute) to
     ``optimize_embedding`` above, so that callers such as the evaluation loop reach the fused path unchanged.  With
     ``train``, ``method.train_iteration`` is rebound (instance attribute) to ``fused_train.train_iteration``: its loss
     always runs as the fused op, while the backbone, ``msssim``, the uncertainty head (``uncertainty``,
     ``uncertainty_modes``) and densification (``densify``) follow their own flags.  With ``render``, ``method.render`` (every evaluation image, video frame and viewer frame) is
     rebound (instance attribute) to ``fused_render.render``: one colour pass, one display composite and one
-    device-to-host copy into pinned memory, the same result arrays."""
+    device-to-host copy into pinned memory, the same result arrays.  With ``resident`` (and ``train``), the training images
+    and masks that fit ``resident_bytes`` (None: half of the device memory free at the first step) are kept on the
+    device, as uint8 where byte-exact and fp32 otherwise, checked and packed there by ``gsr_pack_u8_exact``; each step
+    unpacks its camera from device memory, and the cameras beyond the budget are staged as without the option.  It also
+    implies ``resident_features`` for the uncertainty model (``feature_cache_bytes`` passes through).  The same bits
+    are computed either way; ``disable_method`` frees the store."""
+    if resident:
+        import fused_train
+        kw.setdefault("resident_features", True)
+        method.__dict__[fused_train.RESIDENT_MARK] = None if resident_bytes is None else int(resident_bytes)
     enable(method.model, **kw)
     method.optimize_embedding = types.MethodType(optimize_embedding, method)
     if train:
@@ -493,5 +511,8 @@ def disable_method(method):
     method.__dict__.pop("optimize_embedding", None)
     method.__dict__.pop("train_iteration", None)
     method.__dict__.pop("render", None)
+    if "fused_train" in sys.modules:
+        method.__dict__.pop(sys.modules["fused_train"].RESIDENT_MARK, None)
+        sys.modules["fused_train"].release(method)
     disable(method.model)
     return method
